@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the quantized-linear + paged-attention hot path of mistral.rs on B200.
+"""bench.py — the quantized-linear + paged-attention hot path of mistral.rs on an H100 (sm_90a).
 
 Headline (BASELINE.json configs[1], `--config 2`, the default): Llama-3-8B, GGUF Q4_K_M tensor types,
 decode batch 1, 128-token prompt -> +256 generated tokens, synthetic weights / prompts (SURVEY §8(d)),
@@ -59,7 +59,7 @@ def algorithmic_bytes_per_token(cfg, M, tp=1):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     def __init__(self, gpu_index=0):
         self.proc, self.lines, self.gpu = None, [], gpu_index
@@ -304,21 +304,22 @@ def validate_first_tokens(weights, M, torch, n_tokens=6):
 
 
 # ------------------------------------------------------------------------------------------- config 3
-def bench_prefill_q8(M, torch, dev, peaks, prompt=4096, layers=0):
+def bench_prefill_q8(M, torch, dev, peaks, prompt=4096, layers=0, steps=3, warmup=1, dump=None):
     """BASELINE config 3: Llama-3-8B with Q8_0 blocks everywhere (UQFF q8), one 4096-token prompt.
-    TTFT = embedding -> 32 x (norm, tcgen05 dequant-GEMMs, RoPE, causal prompt attention, KV scatter, GLU) ->
-    lm_head on the last row -> argmax; prefill tok/s = L / TTFT (bench.rs:269-271)."""
+    TTFT = embedding -> 32 x (norm, wgmma dequant-GEMMs, RoPE, causal prompt attention, KV scatter, GLU) ->
+    lm_head on the last row -> argmax; prefill tok/s = L / TTFT (bench.rs:269-271).  `steps` timed prompts (median),
+    after `warmup` untimed ones; `dump` (a dict) receives the last timed prompt's logits and first token."""
     cfg = M.LlamaConfig.llama3_8b(quant="q8_0")
     if layers:
         cfg.n_layers = layers
     w = M.LlamaWeights(cfg, dev, fast_synth=True)
     pre = M.LlamaPrefill(w, max_tokens=prompt)
-    toks = prompt_tokens(0, n=prompt)
-    pre.forward(toks)
+    for it in range(warmup):
+        pre.forward(prompt_tokens(it, n=prompt))
     torch.cuda.synchronize()
     ts = []
-    for it in range(3):
-        toks = prompt_tokens(it + 1, n=prompt)
+    for it in range(steps):
+        toks = prompt_tokens(warmup + it, n=prompt)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         logits = pre.forward(toks)
@@ -326,6 +327,10 @@ def bench_prefill_q8(M, torch, dev, peaks, prompt=4096, layers=0):
         e1.record()
         torch.cuda.synchronize()
         ts.append(e0.elapsed_time(e1) / 1e3)
+    if dump is not None:
+        import numpy as np
+        dump["prefill_logits"] = logits.float().reshape(-1).cpu().numpy()
+        dump["first_token"] = np.array([int(first)], dtype=np.float64)
     ttft = sorted(ts)[len(ts) // 2]
     # attention share, timed alone on the same shapes
     H, KVH, D = cfg.n_heads, cfg.n_kv_heads, cfg.head_dim
@@ -344,9 +349,9 @@ def bench_prefill_q8(M, torch, dev, peaks, prompt=4096, layers=0):
     lin_params = cfg.n_layers * (2 * cfg.hidden * H * D + 2 * cfg.hidden * KVH * D + 3 * cfg.hidden * cfg.inter)
     flop = 2.0 * prompt * lin_params + cfg.n_layers * 2.0 * prompt * prompt * H * D + 2.0 * cfg.vocab * cfg.hidden
     attn_flop = cfg.n_layers * 2.0 * prompt * prompt * H * D
-    tpeak = peaks.get("bf16_tflops_sustained", 1400.0)
+    tpeak = peaks.get("bf16_tflops_sustained", 989.0)
     out = {"workload": "Llama-3-8B Q8_0 (UQFF q8) prefill, 1 x %d tokens, incl. prompt attention, lm_head on the last row" % prompt,
-           "prompt_tokens": prompt, "layers": cfg.n_layers, "ttft_ms": ttft * 1e3, "prefill_tok_s": prompt / ttft,
+           "prompt_tokens": prompt, "layers": cfg.n_layers, "steps": steps, "warmup": warmup, "ttft_ms": ttft * 1e3, "prefill_tok_s": prompt / ttft,
            "tflops": flop / ttft / 1e12, "tensor_peak_tflops": tpeak, "tensor_frac": flop / ttft / 1e12 / tpeak,
            "attention_ms": attn_s * 1e3, "attention_tflops": attn_flop / attn_s / 1e12,
            "linears_ms_est": (ttft - attn_s) * 1e3, "linears_tflops_est": 2.0 * prompt * lin_params / max(ttft - attn_s, 1e-9) / 1e12,
@@ -357,23 +362,25 @@ def bench_prefill_q8(M, torch, dev, peaks, prompt=4096, layers=0):
 
 
 # ------------------------------------------------------------------------------------------- config 4
-def bench_gptq_batch32(torch, dev, peaks, steps=2, layers=0, batch=32):
+def bench_gptq_batch32(torch, dev, peaks, steps=2, layers=0, batch=32, warmup=1, dump=None):
     """BASELINE config 4: Mistral-7B GPTQ int4 (g128, symmetric) decode at batch 32, paged KV block 16,
-    128-token prompts -> +256 tokens, in the HND (FlashInfer) and vLLM cache layouts."""
+    128-token prompts -> +256 tokens, in the HND (FlashInfer) and vLLM cache layouts; `steps` timed generations per
+    layout after `warmup` untimed ones.  `dump` (a dict) receives the last timed HND generation's final token ids and
+    logits."""
     from mistralrs_b200 import gptq_model as G
     cfg = G.GptqConfig.mistral_7b()
     if layers:
         cfg.n_layers = layers
     w = G.GptqWeights(cfg, dev)
-    peak = peaks.get("hbm_gbs", 6650.0)
+    peak = peaks.get("hbm_gbs", 3350.0)
     kv_mean = batch * 2 * cfg.n_kv_heads * cfg.head_dim * 2 * cfg.n_layers * (PROMPT_LEN + GEN_LEN // 2)
     res = {"workload": f"Mistral-7B GPTQ int4 g128 decode batch={batch}, 128-token prompts -> +256 tokens, paged KV block_size=16",
-           "layers": cfg.n_layers, "weight_bytes_per_step": w.nbytes, "kv_bytes_per_step_mean": kv_mean}
+           "layers": cfg.n_layers, "steps": steps, "warmup": warmup, "weight_bytes_per_step": w.nbytes, "kv_bytes_per_step_mean": kv_mean}
     for layout in ("hnd", "vllm"):
         run = G.GptqRunner(w, batch=batch, max_ctx=PROMPT_LEN + GEN_LEN + 16, cache_layout=layout)
         graph = run.capture()
         vals = []
-        for it in range(steps + 1):
+        for it in range(warmup + steps):
             run.reset()
             ptoks = [prompt_tokens(it, case=b) for b in range(batch)]
             for i in range(PROMPT_LEN):
@@ -386,8 +393,12 @@ def bench_gptq_batch32(torch, dev, peaks, steps=2, layers=0, batch=32):
                 graph.replay()
             e1.record()
             torch.cuda.synchronize()
-            if it > 0:
+            if it >= warmup:
                 vals.append(e0.elapsed_time(e1) / 1e3)
+        if dump is not None and layout == "hnd":
+            import numpy as np
+            dump["token_ids"] = run.meta["token_ids"].cpu().numpy().astype(np.float64)
+            dump["last_logits"] = run.logits().float().reshape(-1).cpu().numpy()
         sec = sum(vals) / len(vals)
         step_s = sec / (GEN_LEN - 1)
         res[layout] = {"decode_tok_s": batch * (GEN_LEN - 1) / sec, "ms_per_decode_step": step_s * 1e3,
@@ -402,7 +413,7 @@ def bench_gptq_batch32(torch, dev, peaks, steps=2, layers=0, batch=32):
             lin_s = timed_graph(gg, 10, torch)
             run.step_struct.skip_mask = 0
             res["linears"] = {"ms_per_step": lin_s * 1e3, "achieved_gbs": w.nbytes / lin_s / 1e9, "hbm_frac": w.nbytes / lin_s / 1e9 / peak,
-                              "kernel": "w4a16_kernel<32> (swap-AB tcgen05) + dense lm_head"}
+                              "kernel": "hg_kernel<Int4TileSrc, 32> (swap-AB wgmma) + dense lm_head"}
         del run, graph
     del w
     torch.cuda.empty_cache()
@@ -425,7 +436,12 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the config 3 / config 4 blocks of the default line")
     ap.add_argument("--no-validate", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=0.0, help="bound of one CPU sample (tests); 0: derived from --steps")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (generated token ids, last logits, "
+                         "prompt logits) as DIR/<name>.npy in float32 / float64")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
     if args.impl == "reference":
         return run_reference(args)
     if args.config == 1:
@@ -451,22 +467,33 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (6650.0, "fallback")
+    peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (3350.0, "fallback: H100 SXM data sheet")
+
+    def write_dump(dump):
+        if args.dump_outputs and rank == 0:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, a in dump.items():
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a)
 
     if args.config == 3 and world == 1:
-        pf = bench_prefill_q8(M, torch, dev, peaks, layers=args.layers)
-        print(json.dumps({"metric": "prefill_tok_s", "value": pf["prefill_tok_s"], "unit": "tok/s", "n_gpus": 1, "steps": 3, "warmup": 1,
+        dump = {}
+        pf = bench_prefill_q8(M, torch, dev, peaks, layers=args.layers, steps=args.steps, warmup=args.warmup, dump=dump)
+        write_dump(dump)
+        print(json.dumps({"metric": "prefill_tok_s", "value": pf["prefill_tok_s"], "unit": "tok/s", "n_gpus": 1, "steps": args.steps,
+                          "warmup": args.warmup,
                           "ms_per_step": pf["ttft_ms"], "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-                          "dtype": "bf16 activations x Q8_0 blocks dequantised to bf16 (tcgen05), f32 accumulate", "data": "synthetic",
+                          "dtype": "bf16 activations x Q8_0 blocks dequantised to bf16 (wgmma), f32 accumulate", "data": "synthetic",
                           "config": {"workload": pf["workload"]}, "prefill": pf,
                           "roofline": {"bound": "tensor", "achieved": pf["tflops"], "peak": pf["tensor_peak_tflops"], "unit": "TFLOP/s",
                                        "frac": pf["tensor_frac"], "traffic": None}}))
         return
     if args.config == 4 and world == 1:
-        c4 = bench_gptq_batch32(torch, dev, peaks, steps=max(1, min(args.steps, 3)), layers=args.layers)
+        dump = {}
+        c4 = bench_gptq_batch32(torch, dev, peaks, steps=args.steps, layers=args.layers, warmup=args.warmup, dump=dump)
+        write_dump(dump)
         print(json.dumps({"metric": "decode_tok_s", "value": c4["hnd"]["decode_tok_s"], "unit": "tok/s", "n_gpus": 1, "steps": args.steps,
-                          "warmup": 1, "ms_per_step": c4["hnd"]["ms_per_decode_step"] * (GEN_LEN - 1), "higher_is_better": True,
-                          "scaling": "strong", "vs_baseline": None, "dtype": "f16 activations x int4 (q-8)*s dequantised to f16 (tcgen05), f32 accumulate",
+                          "warmup": args.warmup, "ms_per_step": c4["hnd"]["ms_per_decode_step"] * (GEN_LEN - 1), "higher_is_better": True,
+                          "scaling": "strong", "vs_baseline": None, "dtype": "f16 activations x int4 (q-8)*s dequantised to f16 (wgmma), f32 accumulate",
                           "data": "synthetic", "config": {"workload": c4["workload"]}, "config4": c4,
                           "roofline": {"bound": "hbm", "achieved": c4["linears"]["achieved_gbs"], "peak": peak, "unit": "GB/s",
                                        "frac": c4["linears"]["hbm_frac"], "traffic": None, "peak_source": peak_src}}))
@@ -532,10 +559,14 @@ def main():
         torch.cuda.synchronize()
 
     ttfts = []
+    dump = {}   # the last timed step's outputs (--dump-outputs)
 
-    def generation(it, e2e):
+    def generation(it, e2e, out=None, record=False):
         """one step: the prompt (one prefill pass on a single GPU; token by token through the decode graph
-        under TP), then GEN_LEN tokens.  Returns device-timed seconds of the decode phase."""
+        under TP), then GEN_LEN tokens.  Returns device-timed seconds of the decode phase.  `out` (a dict) receives the
+        prompt logits and the last logits, read after the timed windows; `record` also collects every generated token
+        id, one device copy per token — only for an untimed step."""
+        gen_ids = torch.zeros(GEN_LEN, dtype=torch.int32, device=dev) if record else None
         runner.reset()
         toks = prompt_tokens(it)
         if prefill_runner is not None:
@@ -547,6 +578,8 @@ def main():
             tok_dev.copy_(torch.argmax(logits).to(torch.int32).reshape(1))
             runner.reset(PROMPT_LEN)
             p1.record()
+            if out is not None:   # (after p1: outside the timed prompt window)
+                out["prompt_logits"] = logits.float().reshape(-1).cpu().numpy()
         else:
             for t in toks:
                 pinned_in[0] = t
@@ -556,10 +589,14 @@ def main():
         barrier()
         if prefill_runner is not None:
             ttfts.append(p0.elapsed_time(p1) / 1e3)
+        if record:
+            gen_ids[0].copy_(tok_dev[0])
         e0.record()
         if not e2e:
-            for _ in range(GEN_LEN - 1):
+            for i in range(GEN_LEN - 1):
                 graph.replay()
+                if record:
+                    gen_ids[i + 1].copy_(tok_dev[0])
         else:
             pinned_in.copy_(tok_dev)
             for _ in range(GEN_LEN - 1):
@@ -570,6 +607,10 @@ def main():
                 pinned_in[0] = pinned_out[0]
         e1.record()
         barrier()
+        if out is not None:
+            out["last_logits"] = runner.logits().float().reshape(-1).cpu().numpy()
+        if record:
+            out["token_ids"] = gen_ids.cpu().numpy().astype(np.float64)
         return e0.elapsed_time(e1) / 1e3
 
     def max_over_ranks(x):
@@ -587,7 +628,8 @@ def main():
         sampler = ClockSampler(local)
         if rank == 0:
             sampler.start()
-        ts = [max_over_ranks(generation(args.warmup + i, False)) for i in range(args.steps)]
+        ts = [max_over_ranks(generation(args.warmup + i, False, out=dump if args.dump_outputs and i == args.steps - 1 else None))
+              for i in range(args.steps)]
         return ts, (sampler.stop() if rank == 0 else None)
 
     times, clocks = timed_steps()
@@ -602,6 +644,16 @@ def main():
         if rank == 0:
             clocks["remeasured_after"] = first.get("reasons", [])
     ttft_dev = sorted(ttfts)[len(ttfts) // 2] if ttfts else None
+    if args.dump_outputs:
+        # the generated ids: the same step again, untimed, collecting each token; the step is deterministic, and its
+        # logits must equal the timed step's bit for bit, so these are the ids the timed step produced
+        again = {}
+        generation(args.warmup + args.steps - 1, False, out=again, record=True)
+        for name in ("prompt_logits", "last_logits"):
+            if name in dump and not np.array_equal(dump[name], again[name]):
+                raise AssertionError(f"--dump-outputs: the untimed repeat of the last timed step differs in {name}")
+        dump["token_ids"] = again["token_ids"]
+        write_dump(dump)
     ttfts.clear()
     e2e_times = [max_over_ranks(generation(args.warmup + i, True)) for i in range(max(1, min(args.steps, 2)))]
     ttft_e2e = sorted(ttfts)[len(ttfts) // 2] if ttfts else None
@@ -637,11 +689,6 @@ def main():
     n_gemv = sum(4 if M.tensor_type(cfg, "attn_v", l) == M.tensor_type(cfg, "attn_q", l) else 5 for l in range(cfg.n_layers)) + 1
     achieved = weight_bytes / gemv_s / 1e9
     traffic = None
-    try:   # DRAM bytes per launch from the committed ncu --set full capture of this kernel (single-GPU shapes only)
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        traffic = tr["dram_bytes_per_launch"] if (world == 1 and not big and not args.layers) else None
-    except Exception:
-        pass
 
     # ---- GPU reference arm: the unmodified reference kernels (oracle/_ref) chained as mistral.rs chains them, one
     # CUDA graph per token, same weights, same box (scripts/gpu_reference_chain.py)
@@ -666,7 +713,7 @@ def main():
             sec = e0.elapsed_time(e1) / 1e3
             gpu_ref = {"decode_tok_s": (GEN_LEN - 1) / sec, "launches_per_token": count_graph_kernels(rg),
                        "what": "unmodified reference kernels (mmvq_gguf, rotary, add_rms_norm, reshape_and_cache_flashinfer, flashinfer_decode; "
-                               "built from /root/reference with its own flags) chained per layer as mistral.rs does, CUDA graph per token, "
+                               "built from the reference sources with its own flags) chained per layer as mistral.rs does, CUDA graph per token, "
                                "reference split-KV policy; same synthetic weights, same decode window"}
             del rc_, rg
         except Exception as e:
@@ -717,7 +764,7 @@ def main():
         }
         if ttft_dev is not None:
             out["prompt"] = {"tokens": PROMPT_LEN, "ttft_ms": ttft_dev * 1e3, "prefill_tok_s": PROMPT_LEN / ttft_dev,
-                             "note": "the 128-token prompt of this workload: one prefill pass (tcgen05 dequant-GEMMs + prompt attention + KV scatter) + first sample"}
+                             "note": "the 128-token prompt of this workload: one prefill pass (wgmma dequant-GEMMs + prompt attention + KV scatter) + first sample"}
         if gpu_ref:
             out["gpu_reference"] = gpu_ref
             if "decode_tok_s" in gpu_ref:

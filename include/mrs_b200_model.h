@@ -1,4 +1,4 @@
-/* mrs_b200_model.h — C ABI of the B200-native Llama-family decode layer stack.
+/* mrs_b200_model.h — C ABI of the native Llama-family decode layer stack.
  *
  * This is the host-side caller of the hot path (the role of `Llama::forward` /
  * `Block::forward` in the reference: mistralrs-core/src/models/llama.rs:243-260,475-…),

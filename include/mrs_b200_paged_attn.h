@@ -81,7 +81,7 @@ void update_kv_scales_bf16(void *k, void *v, const long num_elements, float *k_s
 int32_t mrs_swap_blocks(const void *src, void *dst, int64_t block_bytes, const int64_t *pairs, int64_t n_pairs,
                         void *stream);
 
-/* ---- B200-native addition: RoPE + KV write + decode attention + split-KV merge in one launch
+/* ---- native addition: RoPE + KV write + decode attention + split-KV merge in one launch
  * over the HND cache (replaces rotary_embedding_positions + reshape_and_cache_flashinfer +
  * flashinfer_decode + its merge kernel); see csrc/paged_attn.cu.  `pdl`: bit 0 = the launch uses
  * programmatic stream serialisation, bit 1 = interleaved (GPT-J / GGUF llama) RoPE pairing instead
@@ -116,7 +116,7 @@ int32_t mrs_prefill_attention(const void *q, const void *k, const void *v, void 
                               int32_t num_kv_heads, int32_t head_dim, int64_t q_stride, int64_t kv_stride, int64_t o_stride,
                               float softmax_scale, int32_t causal, int32_t window_left, float softcap, uint32_t dtype,
                               void *stream);
-/* mrs_prefill_attention picks between csrc/prefill_attn_tc.cu (tcgen05: S and P in tensor memory, V as an MN-major
+/* mrs_prefill_attention picks between csrc/prefill_attn_tc.cu (wgmma: S and P in registers, V as an MN-major
  * shared-memory operand; head size 128, no window / softcap) and csrc/prefill_attn.cu (mma.sync; everything else).
  * mrs_prefill_attention_tc is the first kernel's own entry: cudaErrorNotSupported (801) when the call does not fit.
  * mrs_prefill_attn_tc_debug(enable, lbo, sbo): enable 0 keeps every call on prefill_attn.cu (A/B, tests); lbo / sbo

@@ -40,7 +40,7 @@ void launch_mmvq_gguf_quantize_q8_1_f32(const void *x, void *vy, int kx, int kx_
 MRS_MMVQ_DECL_T(q4_0) MRS_MMVQ_DECL_T(q4_1) MRS_MMVQ_DECL_T(q5_0) MRS_MMVQ_DECL_T(q5_1) MRS_MMVQ_DECL_T(q8_0)
 MRS_MMVQ_DECL_T(q2_k) MRS_MMVQ_DECL_T(q3_k) MRS_MMVQ_DECL_T(q4_k) MRS_MMVQ_DECL_T(q5_k) MRS_MMVQ_DECL_T(q6_k)
 
-/* ---- B200-native additions (not in the reference; see INTEGRATION.md for the Rust-side use) ---- */
+/* ---- native additions (not in the reference; see INTEGRATION.md for the Rust-side use) ---- */
 
 /* Programmatic dependent launch for the reference-shaped launchers (default off). */
 void mrs_set_pdl(int enabled);
@@ -72,22 +72,14 @@ int mrs_mmvq_fused_qkv_mixed(int type_qk, int type_v, int dt, const void *wq, co
                              const void *x, const void *norm_w, float eps, void *q, void *k, void *v, int K, int nq,
                              int nk, int nv, int b_size, int pdl, void *stream);
 
-/* Prefill GEMM (batch > 8) on tcgen05/TMEM: Y[M,N] = X[M,K] . W[N,K]^T, W in ggml blocks,
+/* Prefill GEMM (batch > 8) on the warpgroup tensor cores (wgmma): Y[M,N] = X[M,K] . W[N,K]^T, W in ggml blocks,
  * X/Y dtype 0 f16 / 1 bf16, K % 64 == 0.  Replaces launch_mmq_quantize_q8_1_* +
  * launch_mmq_gguf_<q> (REF fast_mmq.rs:102-185): no activation quantisation pass. */
 int32_t mrs_mmq_gguf(int32_t ggml_type, const void *w, const void *x, void *y, int32_t M, int32_t N, int32_t K,
                      int32_t dtype, void *stream);
-void mrs_mmq_set_weight_format(int32_t fmt);
-/* mrs_mmq_gguf picks between two tcgen05 kernels: csrc/mmq_ts.cu (swap-AB, dequantised weights as the A operand in
- * tensor memory; Q8_0 / Q4_K / Q6_K, K % 256 == 0, rows a multiple of 16 bytes) and csrc/mmq_tc.cu (everything else).
- * path 0: automatic (default); 1: mmq_tc.cu only.  mrs_mmq_gguf_ts is the first kernel's own entry point: it returns
- * cudaErrorNotSupported (801) when the launch does not fit it. */
-void mrs_mmq_set_path(int32_t path);
-int32_t mrs_mmq_gguf_ts(int32_t ggml_type, const void *w, const void *x, void *y, int32_t M, int32_t N, int32_t K,
-                        int32_t dtype, void *stream);
 
 /* GPTQ / AWQ int4 linear from the raw checkpoint tensors (no Marlin repack) on the same
- * tcgen05 kernel: Y[M,N] f16 = X[M,K] f16 . W; GPTQ qweight [K/8,N] (w = (q-8)*s, optional
+ * wgmma kernel: Y[M,N] f16 = X[M,K] f16 . W; GPTQ qweight [K/8,N] (w = (q-8)*s, optional
  * act-order g_idx [K]), AWQ qweight [K,N/8] + qzeros [K/g,N/8] (w = (q-z)*s); scales f16 [K/g,N].
  * Stands in for marlin_{gptq,awq}_4bit_f16 + {gptq,awq}_marlin_repack (REF gptq/marlin_ffi.rs:6-81). */
 int32_t mrs_gptq_gemm(const void *x, const int32_t *qweight, const void *scales, const int32_t *qzeros,
@@ -114,7 +106,7 @@ int marlin_awq_4bit_bf16(const void *inputs, const int32_t *weight, const void *
 void gptq_marlin_repack(const void *weight, const void *perm, const void *result, int k, int n, int bits, int64_t stream);
 void awq_marlin_repack(const void *weight, const void *perm, const void *result, int k, int n, int bits, int64_t stream);
 
-/* B200-native forms of the same kernel: explicit dtype / scale-column convention, and the dense
+/* Native forms of the same kernel: explicit dtype / scale-column convention, and the dense
  * 16-bit linear (lm_head of GPTQ/AWQ checkpoints at decode batch; REF kernels/gemv/gemv.cu). */
 int32_t mrs_w4a16_gemm(const void *x, const void *w_tiles, const void *scales, const int32_t *qzeros, void *y, int32_t M,
                        int32_t K, int32_t N, int32_t group, int32_t dtype, int32_t scale_perm, void *stream);
@@ -129,7 +121,7 @@ int32_t mrs_dense_linear(const void *x, const void *w, void *y, int32_t M, int32
  * w = scale * q - offset; rows n..padded_n-1 are zero.  The layout inside the three buffers is this library's
  * (csrc/affine.cuh) and only its own marlin_affine_* reads it.
  * matmul: output [m, n] with n the PADDED width the buffers were packed for; `workspace` unused.  Kernel: the
- * tcgen05 dequant GEMM of csrc/mmq_tc.cu with csrc/affine.cuh's dequantiser; any m >= 1, k % 64 == 0. */
+ * wgmma dequant GEMM of csrc/mmq_tc.cu with csrc/affine.cuh's dequantiser; any m >= 1, k % 64 == 0. */
 int32_t mrs_gguf_affine_repack_f16(int32_t format, const void *source, void *payload, void *scales, void *offsets,
                                    int32_t k, int32_t n, int32_t padded_n, uintptr_t stream);
 int32_t mrs_gguf_affine_repack_bf16(int32_t format, const void *source, void *payload, void *scales, void *offsets,

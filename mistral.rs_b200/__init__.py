@@ -1,4 +1,4 @@
-"""mistral.rs_b200 — B200-native (sm_100a) quantized-linear + paged-attention hot path.
+"""mistral.rs_b200 — H100-native (sm_90a) quantized-linear + paged-attention hot path.
 
 The product is `libmrs_b200.so`: hand-written CUDA kernels behind the reference's own
 `extern "C"` symbols (include/*.h).  This Python package is only the thin host-side mirror of
@@ -30,7 +30,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ExtensionMissing(
                 f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback."
+                "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback."
             )
         _lib = ctypes.CDLL(LIB_PATH)
     return _lib

@@ -2,7 +2,7 @@
 // 16-bit scale and offset per 16 / 32 weights, w = scale * q - offset.  Behind the reference's own symbols
 // `mrs_gguf_affine_repack_{f16,bf16}` (REF mistralrs-quant/src/gguf/packed_affine.rs:1436-1457 declarations, :526-585
 // call site: source blocks [n, k/block] -> payload padded_n*k*bits/8 bytes, scales / offsets k/group*padded_n values).
-// The matching GEMM entry points `marlin_affine_{u4,u8}_{f16,bf16}` live in mmq_tc.cu (same tcgen05 kernel as the
+// The matching GEMM entry points `marlin_affine_{u4,u8}_{f16,bf16}` live in mmq_tc.cu (same wgmma kernel as the
 // checkpoint-layout int4 GEMM, with affine.cuh's dequantiser).
 //
 // One thread per (row, 32-weight segment); the per-format arithmetic is affine.cuh, which the CPU suite runs on the
@@ -33,7 +33,7 @@ static int32_t affine_repack(int format, const void *source, void *payload, void
   if (k <= 0 || n <= 0 || padded_n < n || k % sp.block_elems != 0 || k % 64 != 0) return -1;
   if (source == nullptr || payload == nullptr || scales == nullptr || offsets == nullptr) return -1;
   const long long total = (long long)padded_n * (k / 32);
-  const int blocks = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);   // grid-stride over at most 8 CTAs per SM
+  const int blocks = (int)((total + 255) / 256 < 132 * 8 ? (total + 255) / 256 : 132 * 8);   // grid-stride over at most 8 CTAs per SM (132 SMs)
   affine_repack_kernel<<<blocks, 256, 0, st>>>(format, sp, (const uint8_t *)source, (uint8_t *)payload, (uint16_t *)scales, (uint16_t *)offsets, k,
                                                 n, padded_n, bf16);
   return (int32_t)cudaGetLastError();

@@ -336,7 +336,7 @@ __global__ void __launch_bounds__(256) update_kv_scales_kernel(const T *__restri
 template <typename T>
 static void launch_update_kv_scales(void *k, void *v, long n, float *k_scales, float *v_scales, int64_t stream) {
   if (n <= 0) return;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long blocks = (n + 256 * 16 - 1) / (256 * 16);  // >= 16 elements per thread before adding CTAs

@@ -1,8 +1,8 @@
-// common.cuh — shared device helpers for the sm_100a hot-path kernels.
+// common.cuh — shared device helpers for the sm_90a hot-path kernels.
 //
 // Block layouts follow the ggml formats the reference consumes
 // (REF: mistralrs-quant/kernels/mmvq_gguf/mmvq_gguf.cu:134-225).  Everything here is
-// written for sm_100a only: mbarrier + cp.async.bulk (TMA engine, SASS UBLKCP), PDL
+// written for sm_90a only: mbarrier + cp.async.bulk (TMA engine, SASS UBLKCP), PDL
 // (griddepcontrol), 32-wide shuffles.
 #pragma once
 #include <cuda_bf16.h>

@@ -400,9 +400,8 @@ extern "C" int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream) 
       MRS_TRY(mrs_mmvq_fused(L.wq.ggml_type, 2, dt, L.wq.data, L.wk.data, L.wv.data, hidden, L.attn_norm, s->rms_eps,
                              nullptr, s->q, s->k, s->v, H, nq, nkv, nkv, B, 0, pdl, stream));
     } else {
-      // Q4_K_M keeps attn_v in Q6_K on some layers: q∥k fused, v on its own.  (The one-grid form,
-      // mrs_mmvq_fused_qkv_mixed, measured 0.7 % slower here: under PDL the small v launch already
-      // hides behind the q∥k tail, and q∥k loses the CTAs it hands to v.)
+      // Q4_K_M keeps attn_v in Q6_K on some layers: q∥k fused, v on its own.  (Under PDL the small v launch
+      // hides behind the q∥k tail; the one-grid form, mrs_mmvq_fused_qkv_mixed, would take CTAs from q∥k.)
       MRS_TRY(mrs_mmvq_fused(L.wq.ggml_type, 2, dt, L.wq.data, L.wk.data, nullptr, hidden, L.attn_norm, s->rms_eps,
                              nullptr, s->q, s->k, nullptr, H, nq, nkv, 0, B, 0, pdl, stream));
       MRS_TRY(mrs_mmvq_fused(L.wv.ggml_type, 0, dt, L.wv.data, nullptr, nullptr, hidden, L.attn_norm, s->rms_eps,

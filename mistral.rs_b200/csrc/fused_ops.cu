@@ -7,7 +7,7 @@
 //   add_rms_norm_{f32,f16,bf16}                    REF mistralrs-core/src/cuda/sort.cu:403-461,701-727
 //   mrs_rms_norm                                   plain RMSNorm (the reference falls through to
 //                                                  candle_nn::ops::rms_norm — core/src/layers.rs:403-413)
-// In the B200 decode chain these are normally folded into the GEMV prologue/epilogue
+// In the decode chain these are normally folded into the GEMV prologue/epilogue
 // (mrs_mmvq_fused) or the attention kernel; the standalone launchers exist so the library is a
 // drop-in for the reference's FFI and for the prefill path.
 #include "common.cuh"

@@ -3,7 +3,7 @@
 //
 // REF structure mirrored: mistralrs-core/src/models/mistral.rs (Attention / MLP / DecoderLayer
 // forward over `QuantMethod` linears), with the linears on the reference's Marlin symbols
-// (gptq/marlin_ffi.rs) — here the swap-AB tcgen05 kernel of w4a16.cu — and the lm_head as the dense
+// (gptq/marlin_ffi.rs) — here the swap-AB wgmma kernel of w4a16.cu — and the lm_head as the dense
 // 16-bit linear the checkpoint keeps.  Per layer (8 launches):
 //   [RMSNorm] -> fused QKV GEMM -> RoPE + KV write + paged decode attention (one launch, HND; or the
 //   rotary -> reshape_and_cache -> paged_attention_v1 chain for the vLLM layout) -> o_proj GEMM ->

@@ -1,10 +1,10 @@
-// mmvq.cu — streaming decode GEMV (batch 1..8) over ggml quant blocks for sm_100a.
+// mmvq.cu — streaming decode GEMV (batch 1..8) over ggml quant blocks for sm_90a.
 //
 // Drop-in for the reference's `launch_mmvq_gguf_*` C ABI
 // (REF: mistralrs-quant/kernels/mmvq_gguf/mmvq_gguf.cu:1322-1641, declared in
 // mistralrs-quant/src/gguf/ffi.rs and called from src/gguf/fast_mmvq.rs:299,472,682).
 //
-// Design (B200-first, not a port of the dp4a kernel):
+// Design (written for this GPU, not a port of the dp4a kernel):
 //  * The weight matrix is a flat byte stream.  Each CTA owns a contiguous range of rows and a
 //    dedicated producer warp streams it HBM -> shared memory with cp.async.bulk (TMA engine)
 //    into a multi-stage mbarrier ring: one 16-byte-aligned bulk copy per (row, 1024-element K
@@ -27,8 +27,7 @@
 namespace mrs {
 
 // CTA shape: NCW = 8 consumer warps + 1 producer warp, two CTAs per SM; a stage holds 2
-// row-segments per consumer warp.  (A 16-warp one-CTA-per-SM shape measured slower end to end in
-// round 1 — profiles/r01_experiments.md — and was removed.)
+// row-segments per consumer warp.
 constexpr int SSW = 8;  // warps that take part in the RMSNorm sum of squares (fixes its summation order)
 
 constexpr int MAX_STAGES = 12;
@@ -567,7 +566,7 @@ static const DevInfo &query_device() {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     d.max_smem = smem > 0 ? smem : 227 * 1024;
-    d.num_sms = sms > 0 ? sms : 148;
+    d.num_sms = sms > 0 ? sms : 132;
   }
   return d;
 }
@@ -698,9 +697,8 @@ static cudaError_t mmvq_dispatch_dual(int t1, const MmvqParams &pa, int t2, cons
   return cudaErrorNotSupported;
 }
 
-// long streams (lm_head-sized) take K segments twice as long: 2.3 KB copies run the TMA engine at
-// 91 % of the HBM peak where 1.15 KB ones reach 76 %; layer-sized matrices keep the short segments,
-// whose pipeline bubbles are smaller.  Only the k-quants the "M" recipes put on `output`.
+// long streams (lm_head-sized) take K segments twice as long: longer copies keep more bytes in flight per
+// TMA issue; layer-sized matrices keep the short segments, whose pipeline bubbles are smaller.  Only the k-quants the "M" recipes put on `output`.
 template <int T> struct HasLong { static constexpr bool value = (T == MRS_Q4_K || T == MRS_Q6_K); };
 
 template <int T>
@@ -862,7 +860,7 @@ MRS_MMVQ_TYPE(q6_k, MRS_Q6_K)
 // forward declaration (defined below in this file)
 static cudaError_t mmvq_dispatch_dual_entry(int t1, const MmvqParams &pa, int t2, const MmvqParams &pb, cudaStream_t stream);
 
-// ---- B200-native fused entry points (same arithmetic, fewer launches) ------------------------
+// ---- native fused entry points (same arithmetic, fewer launches) ------------------------
 // y = W . q8_1( [rmsnorm_w *] x ) [+ residual]; mode 0 plain, 1 fused GLU, 2 fused QKV.
 // x is raw activations [b_size, K] of dtype `dt`; norm_w may be NULL; residual may be NULL.
 extern "C" int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, const void *w1, const void *w2,

@@ -1,4 +1,4 @@
-// paged_attn.cu — decode attention over a paged KV cache for sm_100a, behind the reference's
+// paged_attn.cu — decode attention over a paged KV cache for sm_90a, behind the reference's
 // C symbols:
 //   paged_attention_v1_{f16,bf16}, paged_attention_v2_{f16,bf16}   (vLLM cache layout)
 //        REF mistralrs-paged-attn/src/cuda/ffi.rs:269-438, pagedattention.cuh:110-485,549-665
@@ -860,7 +860,7 @@ MRS_PAGED(f16, 0u)
 MRS_PAGED(bf16, 1u)
 MRS_PAGED(f32, 2u)
 
-// ---------------------------------------------------------------- B200-native fused decode attention
+// ---------------------------------------------------------------- native fused decode attention
 // RoPE(q, k_new) + KV-cache write + paged decode attention + split-KV merge in ONE launch over
 // the HND cache.  q [B, H*D], k_new/v_new [B, KVH*D] are the raw QKV GEMV outputs; cos/sin
 // [max_pos, D/2]; positions [B] i32; slot_mapping [B] i64; counters: zeroed int32

@@ -1,4 +1,4 @@
-// prefill_attn.cu — causal (var-len) prompt attention over fresh q/k/v tensors for sm_100a.
+// prefill_attn.cu — causal (var-len) prompt attention over fresh q/k/v tensors for sm_90a.
 //
 // The reference runs FlashAttention-2 (an sm80 CuTe kernel) on a fresh prompt:
 //   REF mistralrs-core/src/paged_attention/layers/paged_attention.rs:1413-1475 (prompt path: attention over
@@ -13,7 +13,7 @@
 // ring with cp.async (16-byte copies, two tiles in flight); B fragments come from ldmatrix
 // (transposed for V).  GQA: head h reads KV head h / (H / KVH).  Causal tiles beyond the diagonal
 // are skipped, the diagonal tile is masked in registers; heavy (late) query tiles are scheduled first.
-// Legacy mma.sync path (SASS HMMA).  Head size 128 without window / softcap now runs on prefill_attn_tc.cu (tcgen05);
+// Legacy mma.sync path (SASS HMMA).  Head size 128 without window / softcap now runs on prefill_attn_tc.cu (wgmma);
 // this kernel keeps head size 64, sliding window, softcap, and is the A/B for the other one.
 #include "mma_common.cuh"
 
@@ -243,7 +243,7 @@ extern "C" int32_t mrs_prefill_attention(const void *q, const void *k, const voi
                                          int64_t o_stride, float softmax_scale, int32_t causal, int32_t window_left,
                                          float softcap, uint32_t dtype, void *stream) {
   if (total_tokens <= 0) return 0;
-  {   // the tcgen05 kernel when the call fits it (head size 128, no window, no softcap)
+  {   // the wgmma kernel when the call fits it (head size 128, no window, no softcap)
     const int32_t e = mrs_prefill_attention_tc(q, k, v, out, cu_seqlens, batch, total_tokens, max_seqlen, num_heads, num_kv_heads,
                                                head_dim, q_stride, kv_stride, o_stride, softmax_scale, causal, window_left, softcap,
                                                dtype, stream);

@@ -1,4 +1,4 @@
-// prefill_attn_tc.cu — causal (var-len) prompt attention on the 5th-gen tensor cores (tcgen05 + TMEM), head size 128.
+// prefill_attn_tc.cu — causal (var-len) prompt attention on the warpgroup tensor cores (wgmma), head size 128.
 //
 // Same contract and arithmetic class as prefill_attn.cu (REF mistralrs-core/src/paged_attention/layers/
 // paged_attention.rs:1413-1475 -> flash_attn_varlen; SURVEY §8(f) rank 1): S = QK^T and O = PV on 16-bit MMAs with
@@ -6,20 +6,17 @@
 // the second GEMM.  mrs_prefill_attention routes here for head_dim 128 without window / softcap; prefill_attn.cu
 // (mma.sync) keeps every other case.
 //
-// One CTA = 128 query rows of one (sequence, head), 128-token K/V tiles, 192 threads:
-//   warp 0      TMA: Q once (two SWIZZLE_128B boxes of 64 d), then K and V tiles through two 2-stage rings;
-//   warp 1      MMA issuer (one elected lane, warp-convergent):
-//                 S_j  = Q K_j^T      SS form, both operands K-major in shared memory, M128 N128 K16 x 8
-//                 O   += P_j V_j      TS form: P (16-bit pairs) is the A operand in TENSOR MEMORY, V is the B operand
-//                                     straight from its row-major [token][d] tile = MN-major SWIZZLE_128B
-//                                     (no transpose pass): M128 N128 K16 x 8
-//   warps 2..5  softmax + correction + epilogue, thread = query row = TMEM lane: tcgen05.ld the S row (two passes:
-//               max, then exp2 / sum / pack), tcgen05.st P IN PLACE over the first 64 columns of S (a row is private
-//               to its thread, and chunk c of P lands on columns the thread has already read), rescale O in TMEM only
-//               when some row's maximum moved (warp vote), finally O / l -> global.
-// The per-tile chain S -> softmax -> PV is latency-bound (~5000 clocks for 1024 of tensor work), so the kernel is
-// laid out for TWO CTAs per SM instead of a deeper pipeline inside one: single K / V stages (96 KB of shared memory),
-// 256 TMEM columns — S / P [0,128), O [128,256) — and the other CTA's MMAs fill this one's softmax.
+// One CTA = 128 query rows of one (sequence, head), 128-token K/V tiles, 256 threads (two warpgroups, so that each
+// thread may hold the 64 S, 64 O and 32 P registers of its rows without spilling):
+//   thread 0        TMA: Q once (two SWIZZLE_128B boxes of 64 d), K and V tiles through two 2-stage rings; the
+//                   tiles of step j + 2 are issued once both warpgroups are done with step j;
+//   warpgroups 0, 1 64 query rows each:
+//                     S_j  = Q K_j^T   wgmma m64n128k16 x 8, both operands K-major in shared memory
+//                     softmax on the S accumulators in registers (a row lives in the four threads of a quad)
+//                     O   += P_j V_j   wgmma m64n128k16 x 8 with P as the register A operand (the S accumulator
+//                                      layout IS the A fragment layout) and V straight from its row-major
+//                                      [token][d] tile as an MN-major SWIZZLE_128B operand (no transpose pass)
+//                   then O / l -> global.
 #include "tc_common.cuh"
 
 #include <math.h>
@@ -28,10 +25,10 @@
 namespace mrs {
 
 constexpr int FT_BM = 128, FT_BN = 128, FT_D = 128;
-constexpr int FT_THREADS = 32 * 6;
+constexpr int FT_THREADS = 256;
 constexpr int FT_TILE_BYTES = FT_BN * FT_D * 2;                       // 32 KB: two boxes [128 rows][64 d]
-constexpr int FT_SMEM = 1024 + 3 * FT_TILE_BYTES + 256;              // Q + K + V + barriers
-constexpr uint32_t FT_TCOLS = 256;
+constexpr int FT_STAGES = 2;
+constexpr int FT_SMEM = 1024 + (1 + 2 * FT_STAGES) * FT_TILE_BYTES + 256;   // Q + K ring + V ring + barriers
 
 struct FtParams {
   void *o;
@@ -43,54 +40,21 @@ struct FtParams {
   uint32_t v_lbo, v_sbo;       // MN-major descriptor strides of the V operand, bytes
 };
 
-// shared-memory operand descriptor, SWIZZLE_128B, explicit leading / stride byte offsets
-__device__ __forceinline__ uint64_t umma_desc_sw128_ex(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  const uint64_t addr = (uint64_t)(saddr >> 4) & 0x3FFF;
-  return addr | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_f16_ss_warp(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, e;\n\telect.sync _|e, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void tmem_ld_32x32_nowait(uint32_t taddr, uint32_t *r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t *r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::
-          "r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
 
-__global__ void __launch_bounds__(FT_THREADS, 2)
+template <bool BF>
+__global__ void __launch_bounds__(FT_THREADS, 1)
 prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                        const __grid_constant__ CUtensorMap tmap_v, const FtParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t *q_s = smem, *k_s = smem + FT_TILE_BYTES, *v_s = smem + 2 * FT_TILE_BYTES;
-  uint64_t *bars = (uint64_t *)(smem + 3 * FT_TILE_BYTES);
-  uint64_t *q_full = bars, *k_full = bars + 1, *k_empty = bars + 2, *v_full = bars + 3, *v_empty = bars + 4, *s_full = bars + 5,
-           *p_full = bars + 6, *pv_done = bars + 7;
-  uint32_t *tmem_slot = (uint32_t *)(bars + 8);
+  uint8_t *q_s = smem, *k_s = smem + FT_TILE_BYTES, *v_s = smem + (1 + FT_STAGES) * FT_TILE_BYTES;
+  uint64_t *bars = (uint64_t *)(smem + (1 + 2 * FT_STAGES) * FT_TILE_BYTES);
+  uint64_t *q_full = bars, *k_full = bars + 1, *k_empty = bars + 3, *v_full = bars + 5, *v_empty = bars + 7;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.z, h = blockIdx.y;
@@ -105,162 +69,127 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
   const int kv_end = p.causal ? (q_hi + 1) : len;
   const int nt = (kv_end + FT_BN - 1) / FT_BN;
 
-  if (warp == 0 && lane < 8) {
-    mbar_init(&bars[lane], lane == 6 ? 4u : 1u);      // p_full: the four softmax warps
+  if (tid == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < FT_STAGES; s++) {
+      mbar_init(&k_full[s], 1); mbar_init(&v_full[s], 1); mbar_init(&k_empty[s], 2); mbar_init(&v_empty[s], 2);
+    }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, FT_TCOLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __reduce_max_sync(0xffffffffu, *tmem_slot);
-  const uint32_t t_s = tmem_base, t_p = tmem_base, t_o = tmem_base + 128u;   // P overwrites the head of S
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    mbar_arrive_expect_tx_warp(q_full, FT_TILE_BYTES);
-    tma_load_2d_warp(q_s, &tmap_q, h * FT_D, seq0 + q0, q_full);
-    tma_load_2d_warp(q_s + FT_TILE_BYTES / 2, &tmap_q, h * FT_D + 64, seq0 + q0, q_full);
-    for (int j = 0; j < nt; j++) {
-      const int ph = j & 1;
-      const int row = seq0 + j * FT_BN;
-      mbar_wait(k_empty, ph ^ 1);
-      mbar_arrive_expect_tx_warp(k_full, FT_TILE_BYTES);
-      tma_load_2d_warp(k_s, &tmap_k, kvh * FT_D, row, k_full);
-      tma_load_2d_warp(k_s + FT_TILE_BYTES / 2, &tmap_k, kvh * FT_D + 64, row, k_full);
-      mbar_wait(v_empty, ph ^ 1);
-      mbar_arrive_expect_tx_warp(v_full, FT_TILE_BYTES);
-      tma_load_2d_warp(v_s, &tmap_v, kvh * FT_D, row, v_full);
-      tma_load_2d_warp(v_s + FT_TILE_BYTES / 2, &tmap_v, kvh * FT_D + 64, row, v_full);
+  // K_j and V_j of one step into ring stage j % 2 (TMA, thread 0)
+  auto load_kv = [&](int j) {
+    const int s = j % FT_STAGES, row = seq0 + j * FT_BN;
+    uint8_t *ks = k_s + (size_t)s * FT_TILE_BYTES, *vs = v_s + (size_t)s * FT_TILE_BYTES;
+    mbar_arrive_expect_tx(&k_full[s], FT_TILE_BYTES);
+    tma_load_2d(ks, &tmap_k, kvh * FT_D, row, &k_full[s]);
+    tma_load_2d(ks + FT_TILE_BYTES / 2, &tmap_k, kvh * FT_D + 64, row, &k_full[s]);
+    mbar_arrive_expect_tx(&v_full[s], FT_TILE_BYTES);
+    tma_load_2d(vs, &tmap_v, kvh * FT_D, row, &v_full[s]);
+    tma_load_2d(vs + FT_TILE_BYTES / 2, &tmap_v, kvh * FT_D + 64, row, &v_full[s]);
+  };
+  if (tid == 0) {
+    mbar_arrive_expect_tx(q_full, FT_TILE_BYTES);
+    tma_load_2d(q_s, &tmap_q, h * FT_D, seq0 + q0, q_full);
+    tma_load_2d(q_s + FT_TILE_BYTES / 2, &tmap_q, h * FT_D + 64, seq0 + q0, q_full);
+    for (int j = 0; j < min(nt, FT_STAGES); j++) load_kv(j);
+  }
+
+  // ===================== warpgroups: S, softmax, PV, epilogue =====================
+  const int g = warp >> 2, t = tid & 127;
+  const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);   // this thread's rows r0 and r0 + 8 of the tile
+  const int qg0 = q0 + r0, qg1 = qg0 + 8;
+  const int cq = 2 * (lane & 3);                           // column pair of the accumulator fragments
+  const uint32_t qs = smem_u32(q_s) + (uint32_t)(64 * g) * 128u;
+  float o[64], sacc[64];
+#pragma unroll
+  for (int i = 0; i < 64; i++) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nt; j++) {
+    const int s = j % FT_STAGES, ph = (j / FT_STAGES) & 1;
+    const uint32_t ks = smem_u32(k_s) + (uint32_t)s * FT_TILE_BYTES, vs = smem_u32(v_s) + (uint32_t)s * FT_TILE_BYTES;
+    mbar_wait(&k_full[s], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < 8; c++) {
+      const uint32_t off = (uint32_t)(c >> 2) * (FT_TILE_BYTES / 2);
+      wgmma_ss<128, BF>(sacc, wgmma_desc_sw128(qs + off) + (uint64_t)(2 * (c & 3)), wgmma_desc_sw128(ks + off) + (uint64_t)(2 * (c & 3)),
+                        c ? 1u : 0u);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t fmt = p.bf16 ? 1u : 0u;
-    // c = f32 (bit 4), a / b format (bits 7, 10), b_major = MN (bit 16) for the PV product, N >> 3 at bit 17, M >> 4 at bit 24
-    const uint32_t idesc_s = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(FT_BN >> 3) << 17) | ((uint32_t)(FT_BM >> 4) << 24);
-    const uint32_t idesc_o = (1u << 4) | (fmt << 7) | (fmt << 10) | (1u << 16) | ((uint32_t)(FT_D >> 3) << 17) | ((uint32_t)(FT_BM >> 4) << 24);
-    mbar_wait(q_full, 0);
-    for (int j = 0; j < nt; j++) {
-      const int ph = j & 1;
-      mbar_wait(k_full, ph);
-      if (j > 0) mbar_wait(pv_done, ph ^ 1);           // PV_{j-1} has read P out of the S columns S_j is about to overwrite
-      tc_fence_after();
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold<64>(sacc);
+    if (t == 0) mbar_arrive(&k_empty[s]);
+
+    const int kv0 = j * FT_BN;
+    const int lim0 = min(p.causal ? qg0 : len - 1, len - 1) - kv0, lim1 = min(p.causal ? qg1 : len - 1, len - 1) - kv0;
+    float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < 8; c++) {
-        const uint64_t ad = umma_desc_sw128(q_s + (c >> 2) * (FT_TILE_BYTES / 2)) + (uint64_t)(2 * (c & 3));
-        const uint64_t bd = umma_desc_sw128(k_s + (c >> 2) * (FT_TILE_BYTES / 2)) + (uint64_t)(2 * (c & 3));
-        umma_f16_ss_warp(t_s, ad, bd, idesc_s, c ? 1u : 0u);
+    for (int jj = 0; jj < 16; jj++)
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        const int col = 8 * jj + cq + e;
+        mx0 = fmaxf(mx0, col <= lim0 ? sacc[4 * jj + e] : -INFINITY);
+        mx1 = fmaxf(mx1, col <= lim1 ? sacc[4 * jj + 2 + e] : -INFINITY);
       }
-      umma_commit_warp(s_full);
-      umma_commit_warp(k_empty);
-      mbar_wait(p_full, ph);
-      mbar_wait(v_full, ph);
-      tc_fence_after();
-      const uint32_t vs = smem_u32(v_s);
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0 * p.scale_log2), mn1 = fmaxf(m1, mx1 * p.scale_log2);   // (scale > 0)
+    const float corr0 = (mn0 == m0) ? 1.f : ex2_approx(m0 - mn0), corr1 = (mn1 == m1) ? 1.f : ex2_approx(m1 - mn1);
+    const float ms0 = (mn0 == -INFINITY) ? 0.f : mn0, ms1 = (mn1 == -INFINITY) ? 0.f : mn1;
+    m0 = mn0; m1 = mn1;
+    // p = 2^(s * scale - m), row sums in f32, P rounded to the activation format as the A fragments of the PV MMAs
+    uint32_t pa[32];
+    float rs0 = 0.f, rs1 = 0.f;
 #pragma unroll
-      for (int c = 0; c < 8; c++)     // 16 tokens per MMA: two 8-row groups of 1024 B
-        umma_f16_ts_warp(t_o, t_p + (uint32_t)(8 * c), umma_desc_sw128_ex(vs + (uint32_t)c * 2048u, p.v_lbo, p.v_sbo), idesc_o,
-                         (j | c) ? 1u : 0u);
-      umma_commit_warp(pv_done);
-      umma_commit_warp(v_empty);
+    for (int jj = 0; jj < 16; jj++) {
+      const int col = 8 * jj + cq;
+      const float p00 = (col <= lim0) ? ex2_approx(fmaf(sacc[4 * jj], p.scale_log2, -ms0)) : 0.f;
+      const float p01 = (col + 1 <= lim0) ? ex2_approx(fmaf(sacc[4 * jj + 1], p.scale_log2, -ms0)) : 0.f;
+      const float p10 = (col <= lim1) ? ex2_approx(fmaf(sacc[4 * jj + 2], p.scale_log2, -ms1)) : 0.f;
+      const float p11 = (col + 1 <= lim1) ? ex2_approx(fmaf(sacc[4 * jj + 3], p.scale_log2, -ms1)) : 0.f;
+      rs0 += p00 + p01;
+      rs1 += p10 + p11;
+      // k16 step c = jj / 2: a0 (r0, k lo), a1 (r1, k lo), a2 (r0, k hi), a3 (r1, k hi)
+      pa[4 * (jj >> 1) + 2 * (jj & 1)] = pack_act2_t<BF>(p00, p01);
+      pa[4 * (jj >> 1) + 2 * (jj & 1) + 1] = pack_act2_t<BF>(p10, p11);
     }
-  } else {
-    // ===================== softmax / correction / epilogue: thread = query row =====================
-    const int q4 = warp & 3;
-    const int r = q4 * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(q4 * 32) << 16;
-    const int qg = q0 + r;                                 // row index inside the sequence
-    // m_ref is the exponent's reference point, not necessarily the running maximum: it only moves when a row's
-    // maximum outgrows it by more than 2^8 (then O and l are rescaled).  The quotient O / l does not depend on the
-    // reference, P just lives in [0, 256] instead of [0, 1] — and the O round trip through TMEM, with its wait for the
-    // previous PV, almost never happens (with a plain running maximum some row of a warp moves in most tiles).
-    float m_ref = -INFINITY, l_run = 0.f;
-    for (int j = 0; j < nt; j++) {
-      const int ph = j & 1;
-      const uint32_t ts = t_s + lane_off;
-      const int kv0 = j * FT_BN;
-      const int lim = min(p.causal ? qg : len - 1, len - 1) - kv0;   // columns > lim are masked
-      mbar_wait(s_full, ph);
-      tc_fence_after();
-      // the whole S row in registers: four loads in flight, one wait
-      uint32_t v[128];
-      tmem_ld_32x32_nowait(ts, v);
-      tmem_ld_32x32_nowait(ts + 32u, v + 32);
-      tmem_ld_32x32_nowait(ts + 64u, v + 64);
-      tmem_ld_32x32_nowait(ts + 96u, v + 96);
-      tmem_ld_wait();
-      float mx = -INFINITY;
+    rs0 += __shfl_xor_sync(0xffffffffu, rs0, 1); rs0 += __shfl_xor_sync(0xffffffffu, rs0, 2);
+    rs1 += __shfl_xor_sync(0xffffffffu, rs1, 1); rs1 += __shfl_xor_sync(0xffffffffu, rs1, 2);
+    l0 = l0 * corr0 + rs0;
+    l1 = l1 * corr1 + rs1;
 #pragma unroll
-      for (int i = 0; i < 128; i++) mx = fmaxf(mx, (i <= lim) ? __uint_as_float(v[i]) : -INFINITY);
-      mx *= p.scale_log2;                                   // (scale > 0: max commutes with the scaling)
-      const bool move = (m_ref == -INFINITY) || (mx > m_ref + 8.0f);
-      const float m_use = move ? fmaxf(m_ref, mx) : m_ref;
-      const float corr = (m_use == m_ref) ? 1.f : ex2_approx(m_ref - m_use);   // (m_ref = -inf: 0, nothing accumulated yet)
-      const float msub = (m_use == -INFINITY) ? 0.f : m_use;
-      if (j > 0 && __any_sync(0xffffffffu, corr != 1.f)) {
-        mbar_wait(pv_done, ph ^ 1);                         // (already complete: S_j was issued after it)
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < FT_D; c0 += 32) {
-          uint32_t o[32];
-          tmem_ld_32x32(t_o + lane_off + (uint32_t)c0, o);
-#pragma unroll
-          for (int i = 0; i < 32; i++) o[i] = __float_as_uint(__uint_as_float(o[i]) * corr);
-          tmem_st_32x32(t_o + lane_off + (uint32_t)c0, o);
-        }
-      }
-      // p = 2^(s * scale - m_use), row sum in f32, P rounded to the activation format, written over the head of S
-      float rs = 0.f;
-#pragma unroll
-      for (int c0 = 0; c0 < FT_BN; c0 += 32) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = (c0 + i <= lim) ? ex2_approx(fmaf(__uint_as_float(v[c0 + i]), p.scale_log2, -msub)) : 0.f;
-          const float p1 = (c0 + i + 1 <= lim) ? ex2_approx(fmaf(__uint_as_float(v[c0 + i + 1]), p.scale_log2, -msub)) : 0.f;
-          rs += p0 + p1;
-          if (p.bf16) { const __nv_bfloat162 hh = __floats2bfloat162_rn(p0, p1); pk[i >> 1] = *(const uint32_t *)&hh; }
-          else { const __half2 hh = __floats2half2_rn(p0, p1); pk[i >> 1] = *(const uint32_t *)&hh; }
-        }
-        tmem_st_x16(t_p + lane_off + (uint32_t)(c0 >> 1), pk);
-      }
-      l_run = l_run * corr + rs;
-      m_ref = m_use;
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
+    for (int jj = 0; jj < 16; jj++) {
+      o[4 * jj] *= corr0; o[4 * jj + 1] *= corr0; o[4 * jj + 2] *= corr1; o[4 * jj + 3] *= corr1;
     }
-    // epilogue: O / l -> global, one 256-byte row per thread
-    if (nt > 0) {
-      mbar_wait(pv_done, (nt - 1) & 1);
-      tc_fence_after();
-    }
-    const float inv = (l_run > 0.f) ? 1.f / l_run : 0.f;
-    uint8_t *orow = (uint8_t *)p.o + ((int64_t)(seq0 + qg) * p.o_stride + (int64_t)h * FT_D) * 2;
-#pragma unroll 1
-    for (int c0 = 0; c0 < FT_D; c0 += 32) {
-      uint32_t v[32];
-      if (nt > 0) tmem_ld_32x32(t_o + lane_off + (uint32_t)c0, v);
-      if (qg < len) {
+    mbar_wait(&v_full[s], ph);
+    wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 pk;
-          uint32_t *w = (uint32_t *)&pk;
-#pragma unroll
-          for (int k = 0; k < 4; k++) {
-            const float a = (nt > 0) ? __uint_as_float(v[i + 2 * k]) * inv : 0.f, bq = (nt > 0) ? __uint_as_float(v[i + 2 * k + 1]) * inv : 0.f;
-            if (p.bf16) { const __nv_bfloat162 hh = __floats2bfloat162_rn(a, bq); w[k] = *(const uint32_t *)&hh; }
-            else { const __half2 hh = __floats2half2_rn(a, bq); w[k] = *(const uint32_t *)&hh; }
-          }
-          *(uint4 *)(orow + (size_t)(c0 + i) * 2) = pk;
-        }
-      }
+    for (int c = 0; c < 8; c++)     // 16 tokens per MMA: two 8-row groups of 1024 B
+      wgmma_rs_pv<BF>(o, pa + 4 * c, wgmma_desc_sw128_ex(vs + (uint32_t)c * 2048u, p.v_lbo, p.v_sbo));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_hold<64>(o);
+    if (t == 0) mbar_arrive(&v_empty[s]);
+    if (tid == 0 && j + FT_STAGES < nt) {   // both warpgroups are past step j: its stage takes step j + 2
+      mbar_wait(&k_empty[s], ph);
+      mbar_wait(&v_empty[s], ph);
+      load_kv(j + FT_STAGES);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, FT_TCOLS);
+  // epilogue: O / l -> global, 4-byte pairs
+  const float inv0 = (l0 > 0.f) ? 1.f / l0 : 0.f, inv1 = (l1 > 0.f) ? 1.f / l1 : 0.f;
+#pragma unroll
+  for (int half = 0; half < 2; half++) {
+    const int qg = half ? qg1 : qg0;
+    if (qg >= len) continue;
+    const float inv = half ? inv1 : inv0;
+    uint32_t *orow = (uint32_t *)((uint8_t *)p.o + ((int64_t)(seq0 + qg) * p.o_stride + (int64_t)h * FT_D) * 2);
+#pragma unroll
+    for (int jj = 0; jj < 16; jj++) orow[(8 * jj + cq) >> 1] = pack_act2_t<BF>(o[4 * jj + 2 * half] * inv, o[4 * jj + 2 * half + 1] * inv);
+  }
 }
 
 }  // namespace mrs
@@ -308,7 +237,12 @@ extern "C" int32_t mrs_prefill_attention_tc(const void *q, const void *k, const 
   p.v_lbo = g_ft_lbo; p.v_sbo = g_ft_sbo;
   const int nb = cu_seqlens ? batch : 1, ml = cu_seqlens ? max_seqlen : total_tokens;
   dim3 grid((ml + FT_BM - 1) / FT_BM, num_heads, nb);
-  cudaFuncSetAttribute(prefill_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
-  prefill_attn_tc_kernel<<<grid, FT_THREADS, FT_SMEM, (cudaStream_t)stream>>>(tq, tk, tv, p);
+  if (p.bf16) {
+    cudaFuncSetAttribute(prefill_attn_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
+    prefill_attn_tc_kernel<true><<<grid, FT_THREADS, FT_SMEM, (cudaStream_t)stream>>>(tq, tk, tv, p);
+  } else {
+    cudaFuncSetAttribute(prefill_attn_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
+    prefill_attn_tc_kernel<false><<<grid, FT_THREADS, FT_SMEM, (cudaStream_t)stream>>>(tq, tk, tv, p);
+  }
   return (int32_t)cudaGetLastError();
 }

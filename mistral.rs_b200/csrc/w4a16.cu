@@ -1,57 +1,30 @@
-// w4a16.cu — small-batch W4A16 (GPTQ / AWQ int4) and dense f16/bf16 linear on the 5th-gen tensor
-// cores, "swap-AB": the WEIGHT rows are the MMA's M = 128 and the tokens its N (32 … 256), so a
-// decode batch of 32 fills the tensor core instead of 25 % of a 128-token tile.
+// w4a16.cu — small-batch W4A16 (GPTQ / AWQ int4) and dense f16/bf16 linear on the warpgroup tensor cores
+// (tc_gemm.cuh), "swap-AB": the WEIGHT rows are the wgmma M (two warpgroups x 64) and the tokens its N (32, 64, 128),
+// so a decode batch of 32 fills the instruction instead of a quarter of a 128-token tile.
 //
 // Replaces the reference's Marlin path behind its own symbols
 //   marlin_{gptq,awq}_4bit_{f16,bf16}, {gptq,awq}_marlin_repack     REF mistralrs-quant/src/gptq/marlin_ffi.rs:6-81,
 //   kernels/marlin/marlin_kernel.cuh (one kernel for every m), marlin_repack.cu:255,473
 // and the dense small-batch lm_head of GPTQ checkpoints (REF kernels/gemv/gemv.cu, candle matmul).
 //
-// HBM-bound at m <= 64 (Mistral-7B g128: 3.6 GB of packed weights per step), so the design is a
-// streaming one (per CTA = one 128-row weight tile x one K split, 320 threads, 2 CTAs/SM):
-//   warp 0      producer: cp.async.bulk of the packed int4 rows of the K-step (4 KB, contiguous in the
-//               repacked layout) + TMA tensor load of the activation tile X[NT x 64] (SWIZZLE_128B)
-//   warps 2..9  dequantisers: thread = (weight row, 32-weight half): one LDS.128 of packed nibbles ->
-//               exact (q - 8) [(q - z) for AWQ] in the activation format via the magic-number trick
-//               -> x scale (one rounding, = the reference's dequant) -> K-major 128B-swizzled A tile
-//   warp 1      MMA issuer: tcgen05.mma.cta_group::1.kind::f16, M=128 x N=NT x K=16, D in TMEM
-//   epilogue    (the dequant warps) tcgen05.ld -> [cluster/DSMEM split-K reduction in rank order] ->
-//               y[token][row] in the activation dtype
-// Split-K CTAs of one tile form a thread-block cluster (<= 4): partial accumulators go to the leader's
-// shared memory through DSMEM and are summed in a fixed order — deterministic, no global scratch.
+// HBM-bound at m <= 64 (Mistral-7B g128: 3.6 GB of packed weights per step).  Per thread = (weight row, 32-weight
+// half of a 64-k step): one 16-byte load of packed nibbles (contiguous in the repacked layout) + the group's scale
+// (and AWQ zero point) -> exact (q - 8) [(q - z)] in the activation format via the magic-number trick -> x scale (one
+// rounding, = the reference's dequant) -> the K-major 128B-swizzled A stage.  Dense weights come in through the TMA.
+// When the row tiles alone leave SMs idle, K is split over a thread-block cluster and the partials are added in rank
+// order through DSMEM (deterministic, no global scratch).
 //
 // Repacked weight layout ("mrs int4 tiles", same byte count as the checkpoint tensor so the
 // reference's result buffer [K/16, N*16/8] i32 fits): [K/64][N][32 B]; the 32 bytes of (k-step, row)
 // hold 64 nibbles, word w = k 8w..8w+7 with nibble j < 4 <-> k = 2j and nibble 4+j <-> k = 2j+1 (so
 // that `q & 0x000f000f` yields the f16x2 pair (k, k+1)).
-#include "tc_common.cuh"
+#include "tc_gemm.cuh"
 
 #include <stdio.h>
 
 namespace mrs {
 
-constexpr int WA_BM = 128;      // weight rows per CTA (UMMA M)
-constexpr int WA_BK = 64;       // K per stage
-constexpr int WA_STAGES = 4;
-constexpr int WA_DQ_WARPS = 8;
-constexpr int WA_THREADS = 64 + WA_DQ_WARPS * 32;
-constexpr int WA_A_BYTES = WA_BM * WA_BK * 2;   // 16 KB
-constexpr int WA_RAW_BYTES = WA_BM * 32;        // 4 KB
-
 enum { WA_SRC_INT4 = 0, WA_SRC_DENSE = 1 };
-
-struct WaParams {
-  const uint8_t *wq;       // repacked int4 [K/64][N][32 B]
-  const void *scales;      // [K/group, N] in the activation dtype (columns possibly Marlin-permuted)
-  const int32_t *qzeros;   // AWQ: raw [K/group, N/8] (nibbles in AWQ order) or nullptr
-  void *y;                 // [M, N]
-  int M, N, K, group, dtype;
-  int scale_perm;          // 0: plain columns, 1: Marlin 64-wide permutation, 2: Marlin "single" (32-wide)
-  int m0;                  // first token of this pass
-  int ksteps_per_split;    // K-steps (of 64) per split CTA
-  int raw_stages;          // depth of the packed-weight ring (int4 kernel)
-  int pdl;                 // link of a programmatic-dependent-launch chain: x comes from the upstream grid
-};
 
 // Inverses of the reference's scale-column permutations (REF gptq_cuda.rs:530-540 get_scale_perms):
 // permuted[j] = original[perm[j]], so original column r of a 64- (32-) wide chunk sits at inv(r).
@@ -59,37 +32,6 @@ struct WaParams {
 //   32-wide: perm[8i + j] = 2i + {0,1,8,9,16,17,24,25}[j]   -> inv(r) = 8 ((r % 8) / 2) + 2 (r / 8) + r % 2
 __host__ __device__ __forceinline__ int inv_scale_perm64(int r) { return 8 * (r & 7) + (r >> 3); }
 __host__ __device__ __forceinline__ int inv_scale_perm32(int r) { return 8 * ((r & 7) >> 1) + 2 * (r >> 3) + (r & 1); }
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-__device__ __forceinline__ uint32_t map_to_rank(uint32_t local_smem_addr, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local_smem_addr), "r"(rank));
-  return remote;
-}
-__device__ __forceinline__ void st_cluster_f32_at(uint32_t remote_addr, float v) {
-  asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(remote_addr), "f"(v) : "memory");
-}
-// arrive on another CTA's mbarrier; release at cluster scope orders this thread's earlier remote stores before it
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t remote_bar_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote_bar_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t *bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\tWAITC_LOOP:\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra.uni WAITC_DONE;\n\tbra.uni WAITC_LOOP;\n\tWAITC_DONE:\n\t}" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
 
 // 8 packed nibbles (layout above) -> four 16-bit pairs of (q - zp) * s in the activation format.
 // f16: (q & 0xf) | 0x6400 = 1024 + q exactly; the nibble at bits 4..7 gives 1024 + 16 q, and
@@ -111,196 +53,6 @@ __device__ __forceinline__ void dequant_word_f16(uint32_t q, uint32_t sub_lo, ui
     q >>= 8;
   }
 }
-// ---- shared epilogue: TMEM -> registers -> [cluster split-K reduction] -> y ----------------------
-// Called by ALL threads of the CTA; `epi` marks the 8 epilogue warps (warp ids 2..9), two per TMEM lane
-// quarter.  Split-K: the non-leader CTAs push their partial tile straight into a DEDICATED region of the
-// leader's shared memory (red[rank-1][token][row], never aliased with the operand rings, so no "rings drained"
-// rendezvous is needed) and then arrive, thread by thread with release.cluster, on the leader's `red_bar`;
-// the leader adds the partials in rank order (deterministic).  The only cluster barrier is the start-up one
-// (arrive right after the mbarrier init in the kernel prologue, wait here, long since complete), which
-// guarantees the leader's barrier exists before anybody arrives on it.
-template <int NT>
-__device__ __forceinline__ void wa_epilogue(const WaParams &p, float *red, uint64_t *red_bar, uint64_t *acc_full, uint32_t tmem_base,
-                                            int nk, int ksplit, uint32_t rank, int n0, int rows_valid) {
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  constexpr int CPW = NT / 2;              // columns (tokens) per epilogue warp: two warps share a lane quarter
-  const bool epi = warp >= 2 && warp < 2 + WA_DQ_WARPS;
-  const int q = warp & 3, half = (warp - 2) >> 2;
-  const int row = q * 32 + lane;           // TMEM lane = weight row inside the tile
-  auto ld16 = [&](int col, float *dstv) {
-    uint32_t v[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)col));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; i++) dstv[i] = __uint_as_float(v[i]);
-  };
-  __syncwarp();
-  // PDL: y (and everything written two kernels ago) may only be overwritten once the upstream grid has completed;
-  // this late in the kernel the wait returns at once — and every CTA must pass it so that completion stays transitive
-  if (p.pdl) pdl_wait();
-  if constexpr (NT <= 64) {
-    float acc[CPW];
-    if (epi) {
-      if (nk > 0) {
-        mbar_wait(acc_full, 0);
-        tc_fence_after();
-#pragma unroll
-        for (int c0 = 0; c0 < CPW; c0 += 16) ld16(half * CPW + c0, acc + c0);
-      } else {
-#pragma unroll
-        for (int i = 0; i < CPW; i++) acc[i] = 0.f;
-      }
-    }
-    if (ksplit > 1) {
-      cluster_wait_acquire();              // start-up barrier (every thread of every CTA arrived in the prologue)
-      if (epi && rank != 0) {
-        const uint32_t rbase = map_to_rank(smem_u32(red + ((size_t)(rank - 1) * NT + half * CPW) * WA_BM + row), 0u);
-#pragma unroll
-        for (int i = 0; i < CPW; i++) st_cluster_f32_at(rbase + (uint32_t)i * (WA_BM * 4), acc[i]);
-        mbar_arrive_remote(map_to_rank(smem_u32(red_bar), 0u));
-      }
-      if (epi && rank == 0) {
-        mbar_wait_cluster(red_bar, 0);
-        for (int s = 1; s < ksplit; s++)
-#pragma unroll
-          for (int i = 0; i < CPW; i++) acc[i] += red[((size_t)(s - 1) * NT + half * CPW + i) * WA_BM + row];
-      }
-    }
-    if (epi && rank == 0 && row < rows_valid) {
-      const int nrow = n0 + row;
-#pragma unroll
-      for (int i = 0; i < CPW; i++) {
-        const int tok = p.m0 + half * CPW + i;
-        if (tok < p.M) store_act(p.y, (int64_t)tok * p.N + nrow, acc[i], p.dtype);
-      }
-    }
-  } else {
-    // large token tiles (no split-K): stream the accumulators out 16 columns at a time
-    if (epi && nk > 0) {
-      mbar_wait(acc_full, 0);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < CPW; c0 += 16) {
-        float v[16];
-        ld16(half * CPW + c0, v);
-        if (row < rows_valid) {
-#pragma unroll
-          for (int i = 0; i < 16; i++) {
-            const int tok = p.m0 + half * CPW + c0 + i;
-            if (tok < p.M) store_act(p.y, (int64_t)tok * p.N + n0 + row, v[i], p.dtype);
-          }
-        }
-      }
-    }
-  }
-}
-
-// ---- dense 16-bit weights: A tiles straight from TMA, one ring -------------------------------------
-template <int NT>
-__global__ void __launch_bounds__(WA_THREADS, NT <= 64 ? 2 : 1)
-w16_dense_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w, const WaParams p) {
-  constexpr int X_BYTES = NT * 128;
-  constexpr int STAGE = WA_A_BYTES + X_BYTES;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t *bars = (uint64_t *)(smem + WA_STAGES * STAGE);
-  uint64_t *in_full = bars, *empty = bars + WA_STAGES, *acc_full = bars + 2 * WA_STAGES, *red_bar = acc_full + 1;
-  uint32_t *tmem_slot = (uint32_t *)(red_bar + 1);
-  float *red = (float *)((uint8_t *)bars + 256);   // split-K partials (present only when ksplit > 1)
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n0 = blockIdx.x * WA_BM;
-  const int ksplit = gridDim.y;
-  const uint32_t rank = (ksplit > 1) ? cluster_ctarank() : 0u;
-  const int nk_total = p.K / WA_BK;
-  const int kb0 = (int)rank * p.ksteps_per_split;
-  const int nk = max(0, min(p.ksteps_per_split, nk_total - kb0));
-  const int rows_valid = min(WA_BM, p.N - n0);
-  if (p.pdl && tid == 0) pdl_launch_dependents();
-  if (tid == 0) {
-    for (int s = 0; s < WA_STAGES; s++) { mbar_init(&in_full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
-    mbar_init(red_bar, (uint32_t)(ksplit - 1) * WA_DQ_WARPS * 32u);
-    fence_mbar_init();
-  }
-  constexpr uint32_t TCOLS = NT < 32 ? 32 : NT;
-  if (warp == 1) tmem_alloc(tmem_slot, TCOLS);
-  tc_fence_before();
-  __syncthreads();
-  if (ksplit > 1) cluster_arrive_release();   // start-up cluster barrier; waited on in the epilogue
-  tc_fence_after();
-  // REDUX result lives in a uniform register: the MMA issue loop gets uniform operands (no per-MMA waterfall)
-  const uint32_t tmem_base = __reduce_max_sync(0xffffffffu, *tmem_slot);
-  if (warp == 0) {
-    if (lane == 0) {
-      if (p.pdl) pdl_wait();   // (weights and activations share one stage here: the whole stream waits for the upstream grid)
-      int stage = 0, phase = 0;
-      for (int i = 0; i < nk; i++) {
-        const int kb = kb0 + i;
-        mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t *st = smem + (size_t)stage * STAGE;
-        mbar_arrive_expect_tx(&in_full[stage], X_BYTES + WA_A_BYTES);
-        tma_load_2d(st, &tmap_w, kb * WA_BK, n0, &in_full[stage]);
-        tma_load_2d(st + WA_A_BYTES, &tmap_x, kb * WA_BK, p.m0, &in_full[stage]);
-        if (++stage == WA_STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t fmt = (p.dtype == MRS_BF16) ? 1u : 0u;
-    const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(WA_BM >> 4) << 24);
-    int stage = 0, phase = 0;
-    for (int i = 0; i < nk; i++) {
-      mbar_wait(&in_full[stage], phase);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint8_t *as = smem + (size_t)stage * STAGE, *xs = as + WA_A_BYTES;
-#pragma unroll
-        for (int k = 0; k < WA_BK / 16; k++)
-          umma_f16(tmem_base, umma_desc_sw128(as) + (uint64_t)(2 * k), umma_desc_sw128(xs) + (uint64_t)(2 * k), idesc, (i | k) ? 1u : 0u);
-        umma_commit(&empty[stage]);
-        if (i == nk - 1) umma_commit(acc_full);
-      }
-      __syncwarp();
-      if (++stage == WA_STAGES) { stage = 0; phase ^= 1; }
-    }
-  }
-  wa_epilogue<NT>(p, red, red_bar, acc_full, tmem_base, nk, ksplit, rank, n0, rows_valid);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TCOLS);
-}
-
-// ---- int4 weights: three decoupled rings, A operand in tensor memory --------------------------------
-//   RAW ring (deep: 8 KB stages of packed nibbles, the HBM stream — its depth is what keeps enough bytes in
-//   flight to cover the loaded HBM latency), X ring (activation tiles, L2-resident) and the A ring, which
-//   lives in TENSOR MEMORY: the dequantisers write their 16-bit pairs with tcgen05.st (lane = weight row,
-//   two consecutive-k values per 32-bit column) and the MMA reads A from TMEM (TS form).  No shared-memory
-//   round trip for the dequantised tile: no STS, no generic->async proxy fence (MEMBAR.ALL.CTA), no A bytes
-//   competing with the raw stream for shared memory.
-//   One iteration = 128 k (two 64-k chunks of the repacked layout): dequantiser warp w owns TMEM lane
-//   quarter w & 3 (rows 32 (w & 3) + lane) and chunk (w - 2) >> 2 of the iteration.
-//   warp 0 raw producer | warp 1 MMA | warps 2..9 dequantisers + epilogue | warp 10 X producer
-constexpr int WA_XS = 3, WA_RS_MAX = 12;
-#ifdef MRS_WA_TRACE   // dev build: SM-clock stamps of CTA (0, 0) (scripts/dev_wa_trace.py)
-__device__ long long g_wa_trace[4096];
-#define WA_T(slot) do { if (blockIdx.x == 0 && blockIdx.y == 0 && (threadIdx.x & 31) == 0) g_wa_trace[(slot)] = clock64(); } while (0)
-#else
-#define WA_T(slot) do { } while (0)
-#endif
-constexpr int WA4_BK = 128;                       // k per iteration
-constexpr int WA4_RAW_BYTES = 2 * WA_RAW_BYTES;   // 8 KB of packed nibbles per stage ...
-constexpr int WA4_SC_OFF = WA4_RAW_BYTES;         // ... then up to 4 scale rows [128] of 16 bits (the groups the iteration's 128 k touch)
-constexpr int WA4_ZP_OFF = WA4_SC_OFF + 4 * 256;  // ... then up to 4 AWQ zero-point rows [16] of int32
-constexpr int WA4_STAGE = WA4_ZP_OFF + 4 * 64;    // 9472 B
-constexpr int WA4_THREADS = 64 + WA_DQ_WARPS * 32 + 32;
-template <int NT> struct Wa4Tmem {
-  static constexpr uint32_t COLS = NT <= 64 ? 256u : 512u;        // two CTAs per SM share the 512 columns when NT <= 64
-  static constexpr int AS = (int)((COLS - NT) / 64u) > 6 ? 6 : (int)((COLS - NT) / 64u);   // A stages of 64 columns
-};
-
 // bf16: (q & 0xf) | 0x4300 = 128 + q exactly (the 7-bit mantissa holds the nibble); the subtraction of 128 + zp is
 // exact and the product with the bf16 scale rounds once — the same value as (float)(q - zp) * s rounded to bf16
 __device__ __forceinline__ void dequant_word_bf16_m(uint32_t q, uint32_t sub2, uint32_t s2, uint32_t *out) {
@@ -315,232 +67,53 @@ __device__ __forceinline__ void dequant_word_bf16_m(uint32_t q, uint32_t sub2, u
   }
 }
 
-template <int NT>
-__global__ void __launch_bounds__(WA4_THREADS, NT <= 64 ? 2 : 1)
-w4a16_int4_kernel(const __grid_constant__ CUtensorMap tmap_x, const WaParams p) {
-  constexpr int X_BYTES = NT * 256;                 // two SW128 sub-tiles [NT][64 k]
-  constexpr int AS = Wa4Tmem<NT>::AS;
-  constexpr uint32_t TCOLS = Wa4Tmem<NT>::COLS;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int RS = p.raw_stages;
-  uint8_t *x_ring = smem, *r_ring = x_ring + WA_XS * X_BYTES;
-  uint64_t *bars = (uint64_t *)(r_ring + (size_t)RS * WA4_STAGE);
-  uint64_t *raw_full = bars, *raw_empty = bars + WA_RS_MAX, *x_full = bars + 2 * WA_RS_MAX, *x_empty = x_full + WA_XS,
-           *a_full = x_empty + WA_XS, *a_empty = a_full + 8, *acc_full = a_empty + 8, *red_bar = acc_full + 1;
-  uint32_t *tmem_slot = (uint32_t *)(red_bar + 1);
-  float *red = (float *)((uint8_t *)bars + 512);            // split-K partials (present only when ksplit > 1)
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n0 = blockIdx.x * WA_BM;
-  const int ksplit = gridDim.y;
-  const uint32_t rank = (ksplit > 1) ? cluster_ctarank() : 0u;
-  const int nk_total = p.K / WA_BK;                       // 64-k chunks
-  const int kb0 = (int)rank * p.ksteps_per_split;         // first chunk of this split (even)
-  const int nk = max(0, min(p.ksteps_per_split, nk_total - kb0));
-  const int nit = (nk + 1) >> 1;                          // iterations of two chunks; only the global K tail is half-filled
-  const int rows_valid = min(WA_BM, p.N - n0);
-
-  if (warp == 0) WA_T(0);
-  if (p.pdl && tid == 0) pdl_launch_dependents();
-  // Set-up, split so that the weight stream starts at once: warp 0 initialises the raw ring's barriers (one per
-  // lane), signals the CTA barrier WITHOUT waiting on it (bar.arrive) and goes straight to its copy loop; warp 1
-  // initialises the rest and allocates tensor memory; warps 1..10 meet on the barrier (which also orders warp 0's
-  // initialisation before any consumer's first wait).
-  static_assert(2 * WA_RS_MAX + 2 * WA_XS + 16 + 2 <= 64, "barrier block");
-  uint32_t tmem_base = 0u;
-  if (warp == 0) {
-    if (lane < 2 * WA_RS_MAX) mbar_init(&bars[lane], lane < WA_RS_MAX ? 1u : (uint32_t)WA_DQ_WARPS);
-    fence_mbar_init();
-    __syncwarp();
-    asm volatile("bar.arrive 1, %0;" ::"n"(WA4_THREADS) : "memory");
-    if (ksplit > 1) cluster_arrive_release();   // start-up cluster barrier; waited on in the epilogue
-  } else {
-    if (warp == 1) {
-      // x_full[3] x_empty[3] a_full[8] a_empty[8] acc_full red_bar, in memory order after the raw ring's 24
-      const int b = lane;
-      if (b < 2 * WA_XS + 16 + 2) {
-        uint32_t cnt = 1u;
-        if (b >= 2 * WA_XS && b < 2 * WA_XS + 8) cnt = WA_DQ_WARPS;                                       // a_full
-        if (b == 2 * WA_XS + 17) cnt = ksplit > 1 ? (uint32_t)(ksplit - 1) * WA_DQ_WARPS * 32u : 1u;      // red_bar
-        mbar_init(&x_full[b], cnt);
-      }
-      fence_mbar_init();
-      __syncwarp();
-      tmem_alloc(tmem_slot, TCOLS);
-    }
-    tc_fence_before();
-    asm volatile("bar.sync 1, %0;" ::"n"(WA4_THREADS) : "memory");
-    if (ksplit > 1) cluster_arrive_release();
-    tc_fence_after();
-    // REDUX result lives in a uniform register: the MMA issue loop gets uniform operands (no per-MMA waterfall)
-    tmem_base = __reduce_max_sync(0xffffffffu, *tmem_slot);
-  }
-  const uint32_t tmem_a = tmem_base + (uint32_t)NT;       // A ring: AS stages of 64 columns after the accumulator
-
-  // dequantiser identity
-  const int q4 = warp & 3, hf = (warp - 2) >> 2;   // TMEM lane quarter, which 64-k chunk of the iteration
-  const int r = q4 * 32 + lane;                    // weight row in the tile == TMEM lane
-  const int n = n0 + r;
-  int scol = n;
-  if (p.scale_perm == 1) scol = (n & ~63) + inv_scale_perm64(n & 63);
-  else if (p.scale_perm == 2) scol = (n & ~31) + inv_scale_perm32(n & 31);
-  const int zsh = 4 * ((n & 7) == 0 ? 0 : (n & 7) == 1 ? 4 : (n & 7) == 2 ? 1 : (n & 7) == 3 ? 5 : (n & 7) == 4 ? 2 : (n & 7) == 5 ? 6 : (n & 7) == 6 ? 3 : 7);
-  if (warp == 0) WA_T(1);
-
-  if (warp == 0) {
-    // ===================== raw producer: the HBM stream =====================
-    // The whole warp runs this loop convergently with warp-uniform operands; one elected lane issues each copy
-    // (inside an `if (lane == 0)` region every UBLKCP sits in an ELECT ... BRA.U.ANY loop and the address
-    // arithmetic runs through R2UR waterfalls: ~300 clocks per copy measured — the producer paced the kernel).
-    // Per iteration: the packed nibbles of one or two 64-k chunks, plus the scale row (and AWQ zero-point row) of
-    // every group the iteration's k range touches (one row when group % 128 == 0) — the dequantisers read them
-    // from the stage with LDS; nothing on their path waits for global memory.
-    const uint32_t raw_bytes = (uint32_t)rows_valid * 32u, sc_bytes = (uint32_t)rows_valid * 2u;
-    const uint32_t zp_bytes = p.qzeros ? (uint32_t)rows_valid / 2u : 0u;
-    const uint8_t *w_src = p.wq + ((size_t)kb0 * p.N + n0) * 32;
-    const size_t w_step = (size_t)p.N * 32;
-    const int G = p.group;
-    int k_in_g = (kb0 * WA_BK) % G;
-    const uint8_t *sc_src = (const uint8_t *)p.scales + ((size_t)((kb0 * WA_BK) / G) * p.N + n0) * 2;
-    const uint8_t *zp_src = p.qzeros ? (const uint8_t *)p.qzeros + ((size_t)((kb0 * WA_BK) / G) * (p.N >> 3) + (n0 >> 3)) * 4 : (const uint8_t *)p.scales;
-    const size_t sc_step = (size_t)p.N * 2, zp_step = (size_t)(p.N >> 3) * 4;
-    const uint32_t ring = smem_u32(r_ring);
-    int stage = 0, phase = 0;
-    for (int i = 0; i < nit; i++) {
-      const int nc = min(2, nk - 2 * i);
-      const int x = k_in_g + 64 * nc - 1;                             // last k of the iteration, relative to its first group
-      const int ng = 1 + (x >= G) + (x >= 2 * G) + (x >= 3 * G);      // groups touched (<= 4: 128 k over groups >= 32)
-      const uint32_t st = ring + (uint32_t)stage * WA4_STAGE, bar = smem_u32(&raw_full[stage]);
-      mbar_wait(&raw_empty[stage], phase ^ 1);
-      WA_T(100 + i);
-      mbar_arrive_expect_tx_warp(&raw_full[stage], raw_bytes * (uint32_t)nc + (sc_bytes + zp_bytes) * (uint32_t)ng);
-      bulk_g2s_warp(st, w_src, raw_bytes, bar, 1u);
-      bulk_g2s_warp(st + WA_RAW_BYTES, w_src + w_step, raw_bytes, bar, nc > 1);
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        bulk_g2s_warp(st + WA4_SC_OFF + j * 256, sc_src + j * sc_step, sc_bytes, bar, j < ng);
-        bulk_g2s_warp(st + WA4_ZP_OFF + j * 64, zp_src + j * zp_step, zp_bytes, bar, (j < ng) && zp_bytes != 0u);
-      }
-      w_src += 2 * w_step;
-      k_in_g += WA4_BK;
-      while (k_in_g >= G) { k_in_g -= G; sc_src += sc_step; zp_src += zp_step; }
-      if (++stage == RS) { stage = 0; phase ^= 1; }
-    }
-  } else if (warp == 10) {
-    // ===================== X producer (activation tiles, L2; k beyond K is zero-filled by TMA) =====================
-    if (p.pdl) pdl_wait();   // the activations are the upstream kernel's output; the weight stream (warp 0) never waits
-    int stage = 0, phase = 0;
-    for (int i = 0; i < nit; i++) {
-      mbar_wait(&x_empty[stage], phase ^ 1);
-      mbar_arrive_expect_tx_warp(&x_full[stage], X_BYTES);
-      uint8_t *xs = x_ring + (size_t)stage * X_BYTES;
-      tma_load_2d_warp(xs, &tmap_x, (kb0 + 2 * i) * WA_BK, p.m0, &x_full[stage]);
-      tma_load_2d_warp(xs + NT * 128, &tmap_x, (kb0 + 2 * i + 1) * WA_BK, p.m0, &x_full[stage]);
-      if (++stage == WA_XS) { stage = 0; phase ^= 1; }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: D[128 rows, NT tokens] += A[tmem] . X[smem]^T =====================
-    const uint32_t fmt = (p.dtype == MRS_BF16) ? 1u : 0u;
-    const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(WA_BM >> 4) << 24);
-    int xs_ = 0, xph = 0, as_ = 0, aph = 0;
-    for (int i = 0; i < nit; i++) {
-      mbar_wait(&x_full[xs_], xph);
-      mbar_wait(&a_full[as_], aph);
-      tc_fence_after();
-      WA_T(1000 + 2 * i);
-      {
-        const uint8_t *xs = x_ring + (size_t)xs_ * X_BYTES;
-        const uint64_t d0 = umma_desc_sw128(xs), d1 = umma_desc_sw128(xs + NT * 128);
-        const uint32_t ta = tmem_a + (uint32_t)as_ * 64u;
-#pragma unroll
-        for (int j = 0; j < 8; j++)
-          umma_f16_ts_warp(tmem_base, ta + (uint32_t)(8 * j), (j < 4 ? d0 : d1) + (uint64_t)(2 * (j & 3)), idesc, (i | j) ? 1u : 0u);
-        umma_commit_warp(&a_empty[as_]);
-        umma_commit_warp(&x_empty[xs_]);
-        if (i == nit - 1) umma_commit_warp(acc_full);
-      }
-      WA_T(1001 + 2 * i);
-      if (++xs_ == WA_XS) { xs_ = 0; xph ^= 1; }
-      if (++as_ == AS) { as_ = 0; aph ^= 1; }
-    }
-  } else {
-    // ===================== dequantisers =====================
-    const bool bf = p.dtype == MRS_BF16;
-    const bool has_zp = p.qzeros != nullptr;
-    if (warp == 2) WA_T(2);
-    const int tb = warp == 2 ? 200 : (warp == 9 ? 600 : 3000);
-    (void)tb;
-    // shared-space addresses (LDS, not generic loads)
-    const uint32_t st_base = smem_u32(r_ring);
-    const uint32_t raw_off = (uint32_t)(hf * WA_RAW_BYTES + r * 32);
-    const uint32_t sc_off = (uint32_t)(WA4_SC_OFF + 2 * (scol - n0)), zp_off = (uint32_t)(WA4_ZP_OFF + 4 * (r >> 3));
-    const uint32_t ta_base = tmem_a + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(hf * 32);
-    // which of the iteration's scale rows each 32-weight half of this thread's chunk uses: row = group(k) - group(k_iter)
-    const int G = p.group;
-    auto row_of = [&](int x) { return (x >= G) + (x >= 2 * G) + (x >= 3 * G); };   // x < G + 128, G >= 32
-    int k_in_g = (kb0 * WA_BK) % G;                      // offset of the iteration's first k inside its group
-    int rs_ = 0, rph = 0, as_ = 0, aph = 0;
-    for (int i = 0; i < nit; i++) {
-      uint32_t o[32];
-      const uint32_t st = st_base + (uint32_t)rs_ * WA4_STAGE;
-      const int j0 = row_of(k_in_g + 64 * hf), j1 = row_of(k_in_g + 64 * hf + 32);
-      k_in_g += WA4_BK;
-      while (k_in_g >= G) k_in_g -= G;
-      mbar_wait(&raw_full[rs_], rph);
-      WA_T(tb + 4 * i);
-      if (2 * i + hf < nk) {
-        const uint4 raw0 = lds128(st + raw_off), raw1 = lds128(st + raw_off + 16);
-        const uint32_t sw0 = lds_u16s(st + sc_off + (uint32_t)j0 * 256u), sw1 = lds_u16s(st + sc_off + (uint32_t)j1 * 256u);
-        uint32_t zp0 = 8u, zp1 = 8u;
-        if (has_zp) {
-          zp0 = (lds32(st + zp_off + (uint32_t)j0 * 64u) >> zsh) & 0xFu;
-          zp1 = (lds32(st + zp_off + (uint32_t)j1 * 64u) >> zsh) & 0xFu;
-        }
-        const uint32_t w[8] = {raw0.x, raw0.y, raw0.z, raw0.w, raw1.x, raw1.y, raw1.z, raw1.w};
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const uint32_t s2 = (h ? sw1 : sw0) * 0x00010001u, zp = h ? zp1 : zp0;
-          if (bf) {
-            const uint32_t sub2 = 0x43004300u + zp * 0x00010001u;                                  // bf16x2(128 + zp)
-#pragma unroll
-            for (int c4 = 0; c4 < 4; c4++) dequant_word_bf16_m(w[4 * h + c4], sub2, s2, o + 16 * h + 4 * c4);
-          } else {
-            const uint32_t sub_lo = 0x64006400u + zp * 0x00010001u;                                // f16x2(1024 + zp)
-            const uint32_t sub_hi = (0xD400u + (zp << 4)) * 0x00010001u;                           // f16x2(-(64 + zp)): ulp 1/16 in [64, 128)
-#pragma unroll
-            for (int c4 = 0; c4 < 4; c4++) dequant_word_f16(w[4 * h + c4], sub_lo, sub_hi, s2, o + 16 * h + 4 * c4);
-          }
-        }
-      } else {
-        // half-filled last iteration (K % 128 == 64): this chunk lies beyond K — zero A against TMA's zero X
-#pragma unroll
-        for (int j = 0; j < 32; j++) o[j] = 0u;
-      }
-      WA_T(tb + 4 * i + 1);
-      mbar_wait(&a_empty[as_], aph ^ 1);                 // the MMAs that read this A stage have retired
-      WA_T(tb + 4 * i + 2);
-      tc_fence_after();
-      tmem_st_32x32(ta_base + (uint32_t)as_ * 64u, o);
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&raw_empty[rs_]);                    // the stage's bytes are in registers (and past them): free the slot
-        mbar_arrive(&a_full[as_]);
-      }
-      WA_T(tb + 4 * i + 3);
-      if (++rs_ == RS) { rs_ = 0; rph ^= 1; }
-      if (++as_ == AS) { as_ = 0; aph ^= 1; }
+// ---- weight sources of the warpgroup-MMA GEMM (tc_gemm.cuh) ----------------------------------------
+struct Int4TileSrc {
+  static constexpr bool kTmaA = false;
+  // HBM-bound at decode batch: 16 B per thread and step is 4 KB per CTA; four steps ahead keep 16 KB of weights in flight
+  static constexpr int kAhead = 4;
+  struct Raw { uint4 q; uint32_t s, zp; };
+  const uint8_t *wq;       // repacked int4 [K/64][N][32 B]
+  const uint16_t *scales;  // [K/group, N] in the activation dtype (columns possibly Marlin-permuted)
+  const int32_t *qzeros;   // AWQ: raw [K/group, N/8] (nibbles in AWQ order) or nullptr (zero point 8)
+  int N, group, scale_perm, bf;
+  __device__ __forceinline__ void load(Raw &r, int n, int k) const {
+    r.q = *(const uint4 *)(wq + ((size_t)(k >> 6) * N + n) * 32 + 16 * ((k >> 5) & 1));
+    const int g = k / group;
+    int scol = n;
+    if (scale_perm == 1) scol = (n & ~63) + inv_scale_perm64(n & 63);
+    else if (scale_perm == 2) scol = (n & ~31) + inv_scale_perm32(n & 31);
+    r.s = scales[(size_t)g * N + scol];
+    r.zp = 8u;
+    if (qzeros) {
+      const int c7 = n & 7;
+      const int zsh = 4 * ((c7 & 1) ? 4 + (c7 >> 1) : (c7 >> 1));   // nibble of column n in AWQ order {0,2,4,6,1,3,5,7}
+      r.zp = ((uint32_t)qzeros[(size_t)g * (N >> 3) + (n >> 3)] >> zsh) & 0xFu;
     }
   }
-  if (warp == 2) WA_T(3);
-  wa_epilogue<NT>(p, red, red_bar, acc_full, tmem_base, nk, ksplit, rank, n0, rows_valid);
-  if (warp == 2) WA_T(4);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TCOLS);
-}
+  __device__ __forceinline__ void expand(const Raw &r, int, int, uint32_t *o) const {
+    const uint32_t w[4] = {r.q.x, r.q.y, r.q.z, r.q.w};
+    const uint32_t s2 = r.s * 0x00010001u;
+    if (bf) {
+      const uint32_t sub2 = 0x43004300u + r.zp * 0x00010001u;                                  // bf16x2(128 + zp)
+#pragma unroll
+      for (int c4 = 0; c4 < 4; c4++) dequant_word_bf16_m(w[c4], sub2, s2, o + 4 * c4);
+    } else {
+      const uint32_t sub_lo = 0x64006400u + r.zp * 0x00010001u;                                // f16x2(1024 + zp)
+      const uint32_t sub_hi = (0xD400u + (r.zp << 4)) * 0x00010001u;                           // f16x2(-(64 + zp)): ulp 1/16 in [64, 128)
+#pragma unroll
+      for (int c4 = 0; c4 < 4; c4++) dequant_word_f16(w[c4], sub_lo, sub_hi, s2, o + 4 * c4);
+    }
+  }
+};
+// dense 16-bit weights: A tiles straight from the TMA
+struct DenseSrc {
+  static constexpr bool kTmaA = true;
+  static constexpr int kAhead = 1;
+  struct Raw {};
+  __device__ __forceinline__ void load(Raw &, int, int) const {}
+  __device__ __forceinline__ void expand(const Raw &, int, int, uint32_t *) const {}
+};
 
 // ---------------------------------------------------------------- repack kernels
 // GPTQ checkpoint [K/8, N] i32 (nibble j of word (k8, n) = k 8*k8 + j) -> mrs int4 tiles; `perm`
@@ -587,122 +160,24 @@ __global__ void repack_awq_kernel(const uint32_t *__restrict__ qw, uint32_t *__r
 }
 
 // ---------------------------------------------------------------- host
-// shared-memory plan of the int4 kernel for one (NT, groups) choice: raw stages take what is left of the budget
-struct Wa4Plan { int rs; size_t smem; };
-static Wa4Plan wa4_plan(int NT, int ksplit) {
-  const size_t budget = (NT <= 64) ? (size_t)(227 * 1024) / 2 - 1024 : (size_t)200 * 1024;   // two CTAs per SM for the decode tiles
-  const size_t xring = (size_t)WA_XS * NT * 256;
-  const size_t fixed = 1024 + xring + 512 + (size_t)(ksplit - 1) * NT * WA_BM * 4;
-  int rs = fixed < budget ? (int)((budget - fixed) / WA4_STAGE) : 0;
-  if (rs > WA_RS_MAX) rs = WA_RS_MAX;
-  if (rs < 2) rs = 2;
-  Wa4Plan pl;
-  pl.rs = rs;
-  pl.smem = fixed + (size_t)rs * WA4_STAGE;
-  return pl;
-}
-
-template <int NT, int SRC>
-static cudaError_t launch_wa(const CUtensorMap &tx, const CUtensorMap &tw, WaParams p, int ksplit, cudaStream_t st) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((p.N + WA_BM - 1) / WA_BM, ksplit);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (ksplit > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = 1; attr[na].val.clusterDim.y = ksplit; attr[na].val.clusterDim.z = 1;
-    na++;
-  }
-  if (p.pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    na++;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = na;
-  if constexpr (SRC == WA_SRC_INT4) {
-    auto kern = w4a16_int4_kernel<NT>;
-    const Wa4Plan pl = wa4_plan(NT, ksplit);
-    p.raw_stages = pl.rs;
-    if (pl.smem > 227 * 1024) return cudaErrorInvalidConfiguration;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
-    cfg.blockDim = dim3(WA4_THREADS);
-    cfg.dynamicSmemBytes = pl.smem;
-    return cudaLaunchKernelEx(&cfg, kern, tx, p);
-  } else {
-    auto kern = w16_dense_kernel<NT>;
-    const size_t smem = 1024 + (size_t)WA_STAGES * (WA_A_BYTES + NT * 128) + 256 + (size_t)(ksplit - 1) * NT * WA_BM * 4;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cfg.blockDim = dim3(WA_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    return cudaLaunchKernelEx(&cfg, kern, tx, tw, p);
-  }
-}
-
-// split K over a cluster when the row tiles alone leave SMs idle (two CTAs per SM are resident).  Splits are
-// whole 128-k iterations (an even number of 64-k chunks) so that only the global K tail can be half-filled.
-static int pick_ksplit(int src, int N, int K, int NT, int group) {
-  if (NT > 64) return 1;   // large token tiles stream their epilogue; compute-bound anyway
-  int sms = 148;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int tiles = (N + WA_BM - 1) / WA_BM, nk = K / WA_BK;
-  const int slots = 2 * sms;
-  int ks = 1;
-  for (int c = 2; c <= 4; c *= 2) {
-    const int per = ((nk + c - 1) / c + 1) & ~1;
-    // the split-K partials (c-1 tiles of NT x 128 f32) take their own shared memory: keep >= 4 raw stages beside them
-    const bool fits = (src == WA_SRC_INT4) ? wa4_plan(NT, c).rs >= 4
-                                           : 1024 + (size_t)WA_STAGES * (WA_A_BYTES + NT * 128) + 256 + (size_t)(c - 1) * NT * WA_BM * 4 <= 227 * 1024;
-    if (tiles * c <= slots && per >= 4 && per * (c - 1) < nk && fits) ks = c;
-  }
-  return ks;
-}
-
 static cudaError_t run_wa(int src, const void *x, const void *w, const void *scales, const int32_t *qzeros, void *y, int M,
                           int K, int N, int group, int dtype, int scale_perm, cudaStream_t st, int pdl = 0) {
   if (M <= 0 || N <= 0) return cudaSuccess;
-  if (K % WA_BK != 0 || (dtype != MRS_F16 && dtype != MRS_BF16)) return cudaErrorInvalidValue;
+  if (K % HG_BK != 0 || (dtype != MRS_F16 && dtype != MRS_BF16)) return cudaErrorInvalidValue;
   if (group <= 0) group = K;
   if (src == WA_SRC_INT4 && (group % 32 != 0 || K % group != 0 || N % 8 != 0)) return cudaErrorInvalidValue;
-  if (src == WA_SRC_INT4 && qzeros != nullptr && N % 32 != 0) return cudaErrorInvalidValue;   // zero-point rows travel as 16-byte bulk copies
+  if (src == WA_SRC_INT4 && qzeros != nullptr && N % 32 != 0) return cudaErrorInvalidValue;
   if (((uintptr_t)x & 15) || ((uintptr_t)w & 15)) return cudaErrorMisalignedAddress;
-  CUtensorMap tx, tw;
-  memset(&tw, 0, sizeof tw);
-  for (int m0 = 0; m0 < M; m0 += 256) {
-    const int mt = M - m0 < 256 ? M - m0 : 256;
-    const int NT = mt <= 32 ? 32 : mt <= 64 ? 64 : mt <= 128 ? 128 : 256;
-    if (!tc_make_map_2d(&tx, x, (uint64_t)M, (uint64_t)K, WA_BK, (uint32_t)NT, dtype)) return cudaErrorInvalidValue;
-    if (src == WA_SRC_DENSE && !tc_make_map_2d(&tw, w, (uint64_t)N, (uint64_t)K, WA_BK, WA_BM, dtype)) return cudaErrorInvalidValue;
-    WaParams p = {};
-    p.wq = (const uint8_t *)w; p.scales = scales; p.qzeros = qzeros; p.y = y;
-    p.M = M; p.N = N; p.K = K; p.group = group; p.dtype = dtype; p.scale_perm = scale_perm; p.m0 = m0;
-    p.pdl = (pdl && M <= 256) ? 1 : 0;   // (one pass only: a second token pass would race the first one's output)
-    const int ks = pick_ksplit(src, N, K, NT, group);
-    p.ksteps_per_split = ks > 1 ? (((K / WA_BK + ks - 1) / ks + 1) & ~1) : K / WA_BK;
-    cudaError_t e;
-#define MRS_WA(NTV)                                                                                   \
-  e = (src == WA_SRC_INT4) ? launch_wa<NTV, WA_SRC_INT4>(tx, tw, p, ks, st) : launch_wa<NTV, WA_SRC_DENSE>(tx, tw, p, ks, st)
-    if (NT == 32) MRS_WA(32); else if (NT == 64) MRS_WA(64); else if (NT == 128) MRS_WA(128); else MRS_WA(256);
-#undef MRS_WA
-    if (e != cudaSuccess) return e;
-  }
-  return cudaSuccess;
+  if (src == WA_SRC_DENSE) return hg_run(DenseSrc{}, x, w, y, M, N, K, dtype, pdl, st);
+  const Int4TileSrc s = {(const uint8_t *)w, (const uint16_t *)scales, qzeros, N, group, scale_perm, dtype == MRS_BF16};
+  return hg_run(s, x, nullptr, y, M, N, K, dtype, pdl, st);
 }
 
 }  // namespace mrs
 
 using namespace mrs;
 
-#ifdef MRS_WA_TRACE
-extern "C" int32_t mrs_debug_wa_trace(long long *out, int32_t n) {
-  return (int32_t)cudaMemcpyFromSymbol(out, g_wa_trace, (size_t)n * sizeof(long long));
-}
-#endif
-
-// ---- B200-native entries ---------------------------------------------------------------------
+// ---- native entries ---------------------------------------------------------------------
 // Y[M,N] = X[M,K] . W^T, W = repacked int4 (mrs tiles, see gptq_marlin_repack below); scales
 // [K/group, N] in dtype (0 f16 / 1 bf16), group <= 0: one group; qzeros: AWQ raw zero points or NULL
 // (symmetric, zero point 8); scale_perm: 0 plain, 1/2 Marlin-permuted scale columns.

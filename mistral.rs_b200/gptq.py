@@ -3,9 +3,9 @@ forward_raw :357-398, gptq_linear :451-623).
 
 `GptqMarlinLayer` follows the reference's load and forward flow call for call, through the
 reference's own C symbols (which libmrs_b200.so exports): `{gptq,awq}_marlin_repack` at load,
-`marlin_permute_scales`, then `marlin_{gptq,awq}_4bit_{f16,bf16}` per forward — on the B200 kernel
-behind them (csrc/w4a16.cu: swap-AB tcgen05 GEMM, HBM-bound at decode batch).
-`GptqLayer` consumes the checkpoint tensors as stored (no repack) on the large-tile tcgen05
+`marlin_permute_scales`, then `marlin_{gptq,awq}_4bit_{f16,bf16}` per forward — on our kernel
+behind them (csrc/w4a16.cu: swap-AB wgmma GEMM, HBM-bound at decode batch).
+`GptqLayer` consumes the checkpoint tensors as stored (no repack) on the same wgmma
 dequant-GEMM (`mrs_gptq_gemm`, prefill-sized batches, true act-order semantics).  Only bits == 4
 is implemented.  Like the reference the activations are computed in F16 (`quantized_act_type`)
 and tensor parallelism is rejected (`distributed/layers.rs:776-788`)."""
@@ -139,7 +139,7 @@ class GptqMarlinLayer:
 
 
 def dense_linear(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
-    """y = x . w^T with dense f16/bf16 w [N, K] on the swap-AB tcgen05 kernel (the lm_head of GPTQ/AWQ
+    """y = x . w^T with dense f16/bf16 w [N, K] on the swap-AB wgmma kernel (the lm_head of GPTQ/AWQ
     checkpoints at decode batch; REF kernels/gemv/gemv.cu + candle matmul)."""
     if x.dtype != w.dtype or x.dtype not in (torch.float16, torch.bfloat16):
         raise ValueError("dense_linear: x and w must both be f16 or bf16")

@@ -149,7 +149,7 @@ class GptqWeights:
 class GptqRunner:
     """KV cache + scratch + per-step metadata for a decode batch; drives mrs_gptq_decode_step."""
 
-    def __init__(self, weights: GptqWeights, batch=32, max_ctx=512, cache_layout="hnd", sm_count=148):
+    def __init__(self, weights: GptqWeights, batch=32, max_ctx=512, cache_layout="hnd", sm_count=132):
         cfg, dev, dt = weights.cfg, weights.device, weights.dtype
         self.w, self.cfg, self.dev, self.dt, self.B = weights, cfg, dev, dt, batch
         bs, D, KVH, NH, H = cfg.block_size, cfg.head_dim, cfg.n_kv_heads, cfg.n_heads, cfg.hidden

@@ -298,7 +298,7 @@ def make_paged_kv_tensors(tables, context_lens, block_size, padded_indices_len):
     return indptr, indices[:padded_indices_len], last[:batch]
 
 
-def decode_split_pages(block_size, batch_size, num_kv_heads, max_context_len, sm_count=148):
+def decode_split_pages(block_size, batch_size, num_kv_heads, max_context_len, sm_count=132):
     return int(host_lib().mrs_decode_split_pages(ctypes.c_int64(block_size), ctypes.c_int64(batch_size),
                                                  ctypes.c_int64(num_kv_heads), ctypes.c_int64(sm_count),
                                                  ctypes.c_int64(max_context_len)))

@@ -1,5 +1,5 @@
 """Prefill (batch > 8) quantized GEMM — mirror of `fast_mmq::plain`
-(REF mistralrs-quant/src/gguf/fast_mmq.rs:762-826) on the tcgen05 dequant-GEMM kernel
+(REF mistralrs-quant/src/gguf/fast_mmq.rs:762-826) on the wgmma dequant-GEMM kernel
 (`mrs_mmq_gguf`, csrc/mmq_tc.cu).  Unlike the reference there is no activation quantisation
 pass: activations stay bf16/f16 and weights are dequantised on the fly into shared memory."""
 import ctypes
@@ -31,16 +31,6 @@ def forward(w, xs: torch.Tensor) -> torch.Tensor:
     if rc != 0:
         raise RuntimeError(f"mrs_mmq_gguf failed with cudaError {rc}")
     return out
-
-
-def set_path(path: str):
-    """'auto' (default): csrc/mmq_ts.cu when the launch fits it, else csrc/mmq_tc.cu; 'tc': mmq_tc.cu only (A/B, tests)."""
-    lib().mrs_mmq_set_path(ctypes.c_int({"auto": 0, "tc": 1}[path]))
-
-
-def set_weight_format(fmt: str):
-    """'same' (default: the activations' 16-bit format), 'f16' or 'bf16' for the dequantised weights."""
-    lib().mrs_mmq_set_weight_format(ctypes.c_int({"same": -1, "f16": 0, "bf16": 1}[fmt]))
 
 
 # ---- the reference's entry points over this kernel (REF mistralrs-quant/src/gguf/fast_mmq.rs:760-826).  In the reference the

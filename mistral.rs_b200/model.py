@@ -499,7 +499,7 @@ class LlamaWeights:
         return (t, dt, rows, cols)
 
 
-def runner_split_pages(block_size, batch, n_kv_heads, max_ctx, sm_count=148, min_tokens=64):
+def runner_split_pages(block_size, batch, n_kv_heads, max_ctx, sm_count=132, min_tokens=64):
     """Split-KV chunk (in pages) for the whole-token decode path: enough tiles that
     batch x kv_heads x tiles covers the SMs (one attention CTA per SM), chunks of at least
     `min_tokens`.  The reference's host policy (metadata.rs:61-86, kv_index.decode_split_pages) never
@@ -514,7 +514,7 @@ class LlamaRunner:
     """Owns KV cache + scratch + per-step metadata for a batch of sequences and drives
     mrs_llama_decode_step / mrs_decode_advance (eagerly or as a captured CUDA graph)."""
 
-    def __init__(self, weights: LlamaWeights, batch=1, max_ctx=512, pdl=False, sm_count=148, comm=None,
+    def __init__(self, weights: LlamaWeights, batch=1, max_ctx=512, pdl=False, sm_count=132, comm=None,
                  fused_attention=True, split_policy="sm_fill", split_min_tokens=64, peer_allreduce=None):
         cfg, dev, dt = weights.cfg, weights.device, weights.dtype
         self.w, self.cfg, self.dev, self.dt, self.B = weights, cfg, dev, dt, batch
@@ -654,7 +654,7 @@ class LlamaRunner:
 class LlamaPrefill:
     """Prompt processing (one sequence, positions 0..T-1) composed from the C-ABI ops, in the order
     of the reference's prefill forward (`models/llama.rs` Block::forward with seq_len > 1):
-    RMSNorm -> tcgen05 dequant-GEMMs (`mmq.forward`, the `fast_mmq` path) -> RoPE -> causal prompt
+    RMSNorm -> wgmma dequant-GEMMs (`mmq.forward`, the `fast_mmq` path) -> RoPE -> causal prompt
     attention over the fresh q/k/v (`paged_attn.prefill_attention`, the reference's flash-attn call,
     paged_attention.rs:1413-1475) -> KV scatter into the paged HND cache -> o_proj -> add+RMSNorm ->
     GLU -> down -> add.  TTFT of BASELINE config 3 is the time of `forward` on a 4096-token prompt."""

@@ -205,7 +205,7 @@ def fused_qkv(q_w: QTensor, k_w: QTensor, v_w: QTensor, xs: torch.Tensor):
 
 def mmvq_fused(w0: QTensor, xs: torch.Tensor, *, mode=0, w1=None, w2=None, norm_w=None, eps=1e-5,
                residual=None, activation=GluActivationType.Silu, pdl=False):
-    """B200-native fused entry (`mrs_mmvq_fused`): [RMSNorm] -> Q8_1 -> GEMV -> [GLU | +residual]
+    """Native fused entry (`mrs_mmvq_fused`): [RMSNorm] -> Q8_1 -> GEMV -> [GLU | +residual]
     in ONE launch.  mode 0 plain, 1 fused GLU (w0=gate, w1=up), 2 fused QKV."""
     _, _, k, b_size = _check_common("mrs_mmvq_fused", w0, xs)
     xs = xs.contiguous()
@@ -257,7 +257,7 @@ class GgufMatMul:
     """`QuantMethod` over ggml blocks — mistralrs-quant/src/gguf/mod.rs:44 (`GgufMatMul`).
 
     forward(x): x [..., K] -> [..., N] (+ bias).  Dispatch as gguf/mod.rs:440-479: flat batch
-    1..=8 -> MMVQ; larger batches -> the tcgen05 dequant-GEMM prefill path (`mmq.forward`).
+    1..=8 -> MMVQ; larger batches -> the wgmma dequant-GEMM prefill path (`mmq.forward`).
     """
 
     def __init__(self, w: QTensor, bias: torch.Tensor = None):

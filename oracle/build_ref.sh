@@ -6,8 +6,8 @@
 #
 # Flags follow mistralrs-quant/build.rs:28-43 and mistralrs-paged-attn/build.rs:110-131
 # (-O3 --use_fast_math, half/bf16 operators enabled, -DENABLE_FP8 for paged-attn); the
-# arch is what the reference's build scripts would pick on a B200 (compute cap 100 ->
-# sm_100, no "a" suffix: mistralrs-quant/build.rs:147).
+# arch is what the reference's build scripts would pick on an H100 (compute cap 90 ->
+# sm_90, no "a" suffix: mistralrs-quant/build.rs:147).
 #
 # Usage: oracle/build_ref.sh [target ...]   (default: all fast targets; "flashinfer" is
 # ~10 min and is only built when asked for or when ALL=1).
@@ -23,7 +23,7 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 COMMON=(-std=c++17 -O3 -U__CUDA_NO_HALF_OPERATORS__ -U__CUDA_NO_HALF_CONVERSIONS__
         -U__CUDA_NO_HALF2_OPERATORS__ -U__CUDA_NO_BFLOAT16_CONVERSIONS__
         --expt-relaxed-constexpr --expt-extended-lambda --use_fast_math
-        -gencode arch=compute_100,code=sm_100 --compiler-options -fPIC -shared)
+        -gencode arch=compute_90,code=sm_90 --compiler-options -fPIC -shared)
 Q="$REF/mistralrs-quant/kernels"
 P="$REF/mistralrs-paged-attn/src/cuda"
 C="$REF/mistralrs-core/src/cuda"

@@ -1,4 +1,4 @@
-//! How mistralrs-quant binds the B200 library — SOURCE ONLY (no Rust toolchain exists in the build
+//! How mistralrs-quant binds the H100 library — SOURCE ONLY (no Rust toolchain exists in the build
 //! image, so this file is checked mechanically against include/*.h by tests/test_abi.py, not compiled).
 //!
 //! 1. Nothing changes for the reference-named launchers: `gguf/ffi.rs`, `gptq/marlin_ffi.rs`,
@@ -7,7 +7,7 @@
 //!    (`println!("cargo:rustc-link-lib=dylib=mrs_b200")`), and `GgufMatMul::forward_raw`
 //!    (gguf/mod.rs:440-479) dispatches exactly as before: batch 1..=8 -> `fast_mmvq::*`,
 //!    larger -> `fast_mmq::*`, GPTQ/AWQ -> `marlin_matmul`.
-//! 2. The B200-native fast paths are opt-in wrappers over `mrs_b200_ffi.rs` (generated from the C
+//! 2. The native fast paths are opt-in wrappers over `mrs_b200_ffi.rs` (generated from the C
 //!    headers).  The one below replaces `fast_mmvq::plain` + the preceding RMSNorm + the following
 //!    residual add with a single launch; it keeps `QuantMethod`'s contract (same shapes, dtypes and
 //!    error behaviour) because it is only a different implementation of `forward_raw`.

@@ -61,4 +61,4 @@ if ok_variant:
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 10
         fl = 4.0 * T * T * 128 * H / 2
-        print(f"{'tcgen05' if en else 'mma.sync'}: {ms*1e3:8.1f} us per layer-call  {fl/ms/1e9:7.1f} TFLOP/s (causal flops)", flush=True)
+        print(f"{'wgmma' if en else 'mma.sync'}: {ms*1e3:8.1f} us per layer-call  {fl/ms/1e9:7.1f} TFLOP/s (causal flops)", flush=True)

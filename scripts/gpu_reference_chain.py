@@ -1,4 +1,4 @@
-"""GPU reference arm: the UNMODIFIED reference kernels (oracle/_ref/*.so, compiled from /root/reference by
+"""GPU reference arm: the UNMODIFIED reference kernels (oracle/_ref/*.so, compiled from the reference sources by
 oracle/build_ref.sh with the reference's own flags) chained per decoder layer the way mistral.rs chains them
 (REF mistralrs-core/src/models/llama.rs:243-260 Block::forward, core/src/ops.rs:5036,5081 qkv_projections /
 quantized_ffn -> mistralrs-quant/src/gguf/fast_mmvq.rs:299,472,682), captured in one CUDA graph per token like
@@ -10,7 +10,7 @@ the reference's `pipeline/cuda_graph.rs`:
     -> quantize_q8_1 -> mmvq plain (down_proj)                                          [13-15 launches / layer]
     ... final add_rms_norm -> quantize_q8_1 -> mmvq plain (lm_head) -> argmax
 
-This is "the recompiled Ampere-class kernel path on the same B200" (BASELINE.md §1), not our product: bench.py
+This is "the recompiled Ampere-class kernel path on the same GPU" (BASELINE.md §1), not our product: bench.py
 reports it as `gpu_reference` next to `value`.  Only the KV-index advance, the embedding gather and the argmax
 are ours (plumbing the reference does on the host / in candle)."""
 import ctypes

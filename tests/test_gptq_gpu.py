@@ -1,4 +1,4 @@
-"""GPTQ / AWQ int4 linear (tcgen05 path, raw checkpoint tensors) vs the numpy oracle
+"""GPTQ / AWQ int4 linear (wgmma path, raw checkpoint tensors) vs the numpy oracle
 (w = (q-8)*s symmetric GPTQ incl. act-order g_idx; w = (q-z)*s AWQ), f16 compute.
 Synthetic tensors per SURVEY §8(d): qweight uniform u4, scales f16 2^U(-8,-6), g_idx = k/128 and a
 random permutation (act-order)."""

@@ -1,5 +1,5 @@
 """GPTQ int4 decode stack (mrs_gptq_decode_step: fused QKV / gate||up W4A16 GEMMs on the swap-AB
-tcgen05 kernel, fused RoPE + KV write + paged attention, dense lm_head) vs the CPU oracle stack, in
+wgmma kernel, fused RoPE + KV write + paged attention, dense lm_head) vs the CPU oracle stack, in
 both KV-cache layouts of BASELINE config 4 (HND / FlashInfer and vLLM)."""
 import numpy as np
 import pytest

@@ -1,8 +1,8 @@
 """Pins the CPU oracle (no GPU needed):
   * block decoders vs gguf-py 0.19.0 (tests/golden/gguf_dequant.npz, make_gguf_golden.py) — bit-exact;
   * Q8_1 quantiser, MMVQ arithmetic, fused GLU, RoPE, add_rms_norm, KV-cache scatter and paged
-    attention vs OUTPUTS OF THE UNMODIFIED REFERENCE KERNELS compiled from /root/reference and
-    run on a B200 (tests/golden/ref_golden.npz, make_ref_golden.py)."""
+    attention vs OUTPUTS OF THE UNMODIFIED REFERENCE KERNELS compiled from the reference sources and
+    run on an H100 (tests/golden/ref_golden.npz, make_ref_golden.py)."""
 import os
 
 import numpy as np
@@ -50,7 +50,8 @@ def test_q8_1_quantiser_vs_reference_kernel(ref):
 
 @pytest.mark.parametrize("t", TYPES)
 def test_mmvq_arithmetic_vs_reference_kernel(ref, t):
-    K, N, B = 1024, 24, 2
+    K, B = 1024, 2
+    N = ref[f"mmvq_{t}_y"].shape[1]   # a sample of the reference's output columns (column n uses weight row n)
     want = ref[f"mmvq_{t}_y"]
     got = oracle.mmvq_q8_1(t, ref[f"mmvq_{t}_w"], ref["q8_1_bytes"], K, N, K // 32, B)
     scale = np.abs(want).max()
@@ -121,7 +122,7 @@ def test_exact_product_vs_reference_mmq_kernel(ref, t):
     the reference's own MMQ kernels (`launch_mmq_quantize_q8_1_*` + `launch_mmq_gguf_<q>`, int8 activations): they may
     differ by the reference's activation-quantisation noise only (its self-consistency bound, fast_mmq.rs:1583-1703)."""
     _need(ref, f"mmq_{t}_y")
-    N, K = 256, 1024
+    N, K = ref[f"mmq_{t}_y"].shape[1], 1024   # a sample of the reference's rows and columns (output row m uses input row m)
     exact = oracle.matmul_exact(t, ref[f"mmq_{t}_w"], ref["mmq_x"], K, N)
     want = ref[f"mmq_{t}_y"]
     scale = np.abs(exact).max()

@@ -71,7 +71,7 @@ def test_varlen_batch(cuda):
 
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
 def test_both_kernels_head_128(cuda, dt):
-    """Head size 128 without window / softcap runs on csrc/prefill_attn_tc.cu (tcgen05, S and P in tensor memory);
+    """Head size 128 without window / softcap runs on csrc/prefill_attn_tc.cu (wgmma, S and P in registers);
     mrs_prefill_attn_tc_debug(0, ...) keeps the call on csrc/prefill_attn.cu (mma.sync).  Both against the fp64
     reference, on a ragged multi-tile prompt, causal and not."""
     import ctypes

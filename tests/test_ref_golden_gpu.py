@@ -32,7 +32,8 @@ def test_q8_1_bytes_identical(cuda, ref):
 
 @pytest.mark.parametrize("t", TYPES)
 def test_mmvq_plain_and_glu(cuda, ref, t):
-    K, N, B = 1024, 24, 2
+    K, B = 1024, 2
+    N = ref[f"mmvq_{t}_y"].shape[1]
     w = quant.QTensor(to_dev(ref[f"mmvq_{t}_w"].reshape(-1), cuda), t, (N, K))
     up = quant.QTensor(to_dev(ref[f"mmvq_{t}_up"].reshape(-1), cuda), t, (N, K))
     y = quant.plain(w, to_dev(ref["mmvq_x"], cuda, "f32") if False else to_dev(ref["mmvq_x"], cuda, "bf16").float()).cpu().numpy()
@@ -105,7 +106,7 @@ def _need(ref, key):
 
 @pytest.mark.parametrize("t", ["q4_k", "q6_k", "q8_0"])
 def test_prefill_gemm_vs_reference_mmq(cuda, ref, t):
-    """`mrs_mmq_gguf` (bf16 activations x dequantised weights on tcgen05) against the output of the
+    """`mrs_mmq_gguf` (bf16 activations x dequantised weights on wgmma) against the output of the
     reference's own MMQ kernels (`launch_mmq_quantize_q8_1_*` + `launch_mmq_gguf_<q>`, int8
     activations).  The two differ by the reference's activation quantisation noise (its own
     self-consistency bound is 5e-3 relative, fast_mmq.rs:1583-1703); both must sit inside that
@@ -113,10 +114,15 @@ def test_prefill_gemm_vs_reference_mmq(cuda, ref, t):
     import oracle
     from mistralrs_b200 import mmq
     _need(ref, f"mmq_{t}_y")
-    M, N, K = 64, 256, 1024
-    wb, x, want = ref[f"mmq_{t}_w"], ref["mmq_x"], ref[f"mmq_{t}_y"]
+    # the stored vectors are a sample of the reference's 64 x 256 product: rows `mmq_rows` of x and y, the first weight
+    # rows; the other token rows of the 64-token launch are zero
+    M, K = 64, 1024
+    wb, x, want, rows = ref[f"mmq_{t}_w"], ref["mmq_x"], ref[f"mmq_{t}_y"], ref["mmq_rows"]
+    N = want.shape[1]
+    xf = np.zeros((M, K), np.float32)
+    xf[rows] = x
     w = quant.QTensor(to_dev(wb.reshape(-1), cuda), t, (N, K))
-    got = mmq.forward(w, to_dev(x, cuda, "bf16")).float().cpu().numpy()
+    got = mmq.forward(w, to_dev(xf, cuda, "bf16")).float().cpu().numpy()[rows]
     exact = oracle.matmul_exact(t, wb, x, K, N)
     scale = np.abs(exact).max()
     e_ref, e_ours = np.abs(want - exact).max() / scale, np.abs(got - exact).max() / scale
@@ -133,8 +139,11 @@ def test_gptq_vs_reference_marlin(cuda, ref, tag, M):
     _need(ref, f"marlin_{tag}_y")
     assert int(ref[f"marlin_{tag}_rc"]) == 0
     x, qw, sc, want = ref[f"marlin_{tag}_x"], ref[f"marlin_{tag}_qweight"], ref[f"marlin_{tag}_scales"], ref[f"marlin_{tag}_y"]
+    rows = ref[f"marlin_{tag}_rows"] if f"marlin_{tag}_rows" in ref.files else np.arange(M)
+    xf = np.zeros((M, x.shape[1]), np.float16)   # stored: a sample of the token rows; the others are zero
+    xf[rows] = x
     layer = gptq.GptqLayer(torch.from_numpy(qw).to(cuda), torch.from_numpy(sc).to(cuda), group_size=128)
-    got = layer.forward_raw(torch.from_numpy(x).to(cuda)).float().cpu().numpy()
+    got = layer.forward_raw(torch.from_numpy(xf).to(cuda)).float().cpu().numpy()[rows]
     scale = np.abs(want).max()
     assert np.abs(got - want).max() <= 2.0 ** -10 * scale + 1e-6, float(np.abs(got - want).max() / scale)
 

@@ -72,7 +72,7 @@ def test_uqff_llama_decode_matches_oracle(cuda, tmp_path):
 
 
 def test_prefill_composition_matches_oracle(cuda):
-    # prompt processing through mmq (tcgen05 dequant-GEMM) + rope + KV scatter + causal attention via
+    # prompt processing through mmq (wgmma dequant-GEMM) + rope + KV scatter + causal attention via
     # the paged decode kernel, against the oracle stepping token by token with EXACT linears
     cfg = M.LlamaConfig.tiny_test(quant="q4_k_m", n_layers=2)
     w = M.LlamaWeights(cfg, cuda, keep_host=True)            # bf16 (f16 overflows on the synthetic 2-layer model)

@@ -7,11 +7,8 @@
     multiplies by), tolerance = one output rounding (2^-11 f16 / 2^-8 bf16) + f32 accumulation slack;
   * and the reference's own bar against the plain dequantised weights: max |diff| <= 0.08, mean <= 0.01.
 
-STATUS: this file landed after the round's GPU budget was spent — the per-format arithmetic is verified on the CPU
-(tests/test_affine_host.py runs the same csrc/affine.cuh code on the host) and the GEMM is the already-verified
-tcgen05 kernel of the checkpoint-layout int4 path with a different dequantiser, but none of it has been RUN on a
-B200 yet.  The tests are therefore marked xfail(strict=False): a pass shows up as XPASS, a failure does not gate the rest of
-the suite.  The file sorts last for the same reason."""
+The GEMM is the warpgroup-MMA kernel of the checkpoint-layout int4 path with the affine dequantiser; the per-format
+arithmetic is also checked on the CPU (tests/test_affine_host.py runs the same csrc/affine.cuh code on the host)."""
 import numpy as np
 import pytest
 import torch
@@ -20,7 +17,7 @@ import oracle
 from oracle import affine_np as A
 from mistralrs_b200 import packed_affine as PA
 
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="a5 landed after the GPU budget was spent: not yet run on hardware")]
+pytestmark = pytest.mark.gpu
 
 TORCH = {"f16": torch.float16, "bf16": torch.bfloat16}
 
