@@ -116,6 +116,37 @@ int32_t mrs_prefill_attention(const void *q, const void *k, const void *v, void 
                               int32_t num_kv_heads, int32_t head_dim, int64_t q_stride, int64_t kv_stride, int64_t o_stride,
                               float softmax_scale, int32_t causal, int32_t window_left, float softcap, uint32_t dtype,
                               void *stream);
+/* ---- prompt attention of new query tokens over K/V already in the HND page cache: prefix-cache hits and chunked
+ * prompts (REF paged_attention.rs:973-1200 `try_prefix_gather_prefill`, plan FlashAttentionPaged ->
+ * flash_attn_varlen_paged_windowed, mistralrs-flash-attn/src/flash.rs:979-1010).
+ *   Shapes     q [total_q, H, D] with token stride q_stride (elements), out [total_q, H, D] with o_stride; key_cache /
+ *              value_cache HND [num_blocks, KVH, page_size, D] in q's 16-bit dtype (0 f16 / 1 bf16).
+ *   Sequences  sequence b owns query rows cu_seqlens_q[b] .. cu_seqlens_q[b+1] and kv_len = cu_seqlens_k[b+1] -
+ *              cu_seqlens_k[b] keys (both cumulative, device i32 [batch + 1]); key j sits at slot
+ *              block_table[b * block_table_stride + j / page_size] * page_size + j % page_size.
+ *   Positions  query i of sequence b is at absolute position kv_len - q_len + i: causal masking is aligned bottom-right;
+ *              window_left >= 0 keeps keys j >= pos - window_left; causal = 0 sees all kv_len keys.  softcap <= 0: off.
+ *   Ordering   the new tokens' K/V are already in the cache (the caller scatters them first); kv_len >= q_len.
+ *   Table      entries at or past ceil(kv_len / page_size) are never read (rows may be padded with anything); cache
+ *              rows past kv_len, including stale rows of the last page, contribute exactly zero.
+ *   Support    head_dim 64 | 128, page_size 8 | 16 | 32, GQA, var-len batches; no FP8 cache, ALiBi or sinks.
+ *   Errors     returns a cudaError_t; stream-ordered, no allocation, no synchronisation (graph-capturable).
+ * Head 128 without window / softcap runs on the wgmma kernel (mrs_prefill_attention_paged_tc, cudaErrorNotSupported
+ * when the call does not fit), everything else on the mma.sync one; mrs_prefill_attn_tc_debug(0, ...) applies here too. */
+int32_t mrs_prefill_attention_paged(const void *q, const void *key_cache, const void *value_cache, void *out,
+                                    const int32_t *block_table, int32_t block_table_stride, const int32_t *cu_seqlens_q,
+                                    const int32_t *cu_seqlens_k, int32_t batch, int32_t total_q, int32_t max_seqlen_q,
+                                    int32_t max_seqlen_k, int32_t num_blocks, int32_t num_heads, int32_t num_kv_heads,
+                                    int32_t head_dim, int32_t page_size, int64_t q_stride, int64_t o_stride,
+                                    float softmax_scale, int32_t causal, int32_t window_left, float softcap, uint32_t dtype,
+                                    void *stream);
+int32_t mrs_prefill_attention_paged_tc(const void *q, const void *key_cache, const void *value_cache, void *out,
+                                       const int32_t *block_table, int32_t block_table_stride, const int32_t *cu_seqlens_q,
+                                       const int32_t *cu_seqlens_k, int32_t batch, int32_t total_q, int32_t max_seqlen_q,
+                                       int32_t max_seqlen_k, int32_t num_blocks, int32_t num_heads, int32_t num_kv_heads,
+                                       int32_t head_dim, int32_t page_size, int64_t q_stride, int64_t o_stride,
+                                       float softmax_scale, int32_t causal, int32_t window_left, float softcap,
+                                       uint32_t dtype, void *stream);
 /* mrs_prefill_attention picks between csrc/prefill_attn_tc.cu (wgmma: S and P in registers, V as an MN-major
  * shared-memory operand; head size 128, no window / softcap) and csrc/prefill_attn.cu (mma.sync; everything else).
  * mrs_prefill_attention_tc is the first kernel's own entry: cudaErrorNotSupported (801) when the call does not fit.

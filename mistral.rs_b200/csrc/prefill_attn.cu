@@ -15,6 +15,10 @@
 // are skipped, the diagonal tile is masked in registers; heavy (late) query tiles are scheduled first.
 // Legacy mma.sync path (SASS HMMA).  Head size 128 without window / softcap now runs on prefill_attn_tc.cu (wgmma);
 // this kernel keeps head size 64, sliding window, softcap, and is the A/B for the other one.
+//
+// PAGED = true reads K/V from the HND page cache [num_blocks, KVH, page, D] (mrs_prefill_attention_paged): each
+// cp.async row looks its page up in the sequence's block table; rows at or past kv_len are zero-filled and their
+// page is never looked up.  Query i of a sequence sits at key position kv_len - q_len + i (bottom-right causal).
 #include "mma_common.cuh"
 
 #include <stdio.h>
@@ -33,9 +37,12 @@ struct FaParams {
   float softcap;               // <= 0: off (applied to scale * qk, like the reference's flash-attn softcap)
   float softmax_scale;
   int causal, window_left;     // window_left < 0: off
+  const int32_t *cu_seqlens_k; // paged: [B + 1] cumulative key counts (cu_seqlens then holds the query rows)
+  const int32_t *block_table;  // paged: [B][bt_stride] page ids
+  int bt_stride, page_shift;   // paged: page = 1 << page_shift tokens
 };
 
-template <typename T, int D>
+template <typename T, int D, bool PAGED>
 __global__ void __launch_bounds__(FA_THREADS, 1) prefill_attn_kernel(const FaParams p) {
   constexpr int KSTEPS = D / 16;        // k-steps of QK^T
   constexpr int DT = D / 8;             // 8-wide n-tiles of the output
@@ -50,27 +57,36 @@ __global__ void __launch_bounds__(FA_THREADS, 1) prefill_attn_kernel(const FaPar
   const int kvh = h / (p.H / p.KVH);
   int seq0 = 0, len = p.T;
   if (p.cu_seqlens != nullptr) { seq0 = p.cu_seqlens[b]; len = p.cu_seqlens[b + 1] - seq0; }
+  int kv_len = len;                                  // keys of the sequence; query i sits at key kv_len - len + i
+  if constexpr (PAGED) kv_len = p.cu_seqlens_k[b + 1] - p.cu_seqlens_k[b];
+  const int off = kv_len - len;
   const int ntile_q = (len + FA_BM - 1) / FA_BM;
   const int qt = ntile_q - 1 - (int)blockIdx.x;     // heavy tiles first
   if (qt < 0) return;
   const int q0 = qt * FA_BM;
   const T *qg = (const T *)p.q + (int64_t)seq0 * p.q_stride + (int64_t)h * D;
-  const T *kg = (const T *)p.k + (int64_t)seq0 * p.kv_stride + (int64_t)kvh * D;
-  const T *vg = (const T *)p.v + (int64_t)seq0 * p.kv_stride + (int64_t)kvh * D;
+  const int64_t kv_base = PAGED ? ((int64_t)kvh * D << p.page_shift) : (int64_t)seq0 * p.kv_stride + (int64_t)kvh * D;
+  const T *kg = (const T *)p.k + kv_base;
+  const T *vg = (const T *)p.v + kv_base;
+  // elements from kg / vg to key j < kv_len of a paged sequence
+  auto page_off = [&](int j) -> int64_t {
+    const int64_t blk = p.block_table[(int64_t)b * p.bt_stride + (j >> p.page_shift)];
+    return ((blk * p.KVH << p.page_shift) + (j & ((1 << p.page_shift) - 1))) * D;
+  };
   T *og = (T *)p.o + (int64_t)seq0 * p.o_stride + (int64_t)h * D;
 
   // KV range of this query tile
   const int q_hi = min(len, q0 + FA_BM) - 1;                               // last query row
-  const int kv_end = p.causal ? (q_hi + 1) : len;
-  const int kv_begin = (p.window_left >= 0) ? max(0, q0 - p.window_left) / FA_BN * FA_BN : 0;
+  const int kv_end = p.causal ? (off + q_hi + 1) : kv_len;
+  const int kv_begin = (p.window_left >= 0) ? max(0, off + q0 - p.window_left) / FA_BN * FA_BN : 0;
   const int nt = (kv_end - kv_begin + FA_BN - 1) / FA_BN;
 
   auto load_tile = [&](int t, int buf) {
     const int t0 = kv_begin + t * FA_BN;
     for (int c = tid; c < FA_BN * CPR; c += FA_THREADS) {
       const int row = c / CPR, ch = c % CPR;
-      const bool ok = t0 + row < len;
-      const int64_t goff = (int64_t)(ok ? t0 + row : 0) * p.kv_stride + ch * 8;
+      const bool ok = t0 + row < kv_len;
+      const int64_t goff = PAGED ? (ok ? page_off(t0 + row) : 0) + ch * 8 : (int64_t)(ok ? t0 + row : 0) * p.kv_stride + ch * 8;
       cp_async16(sk[buf] + tile_off<D>(row, ch), kg + goff, ok);
       cp_async16(sv[buf] + tile_off<D>(row, ch), vg + goff, ok);
     }
@@ -133,7 +149,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1) prefill_attn_kernel(const FaPar
     }
 
     // ---- scale, soft-cap, mask, online softmax (base 2)
-    const bool need_mask = (t0 + FA_BN > kv_end) || (p.causal && t0 + FA_BN - 1 > q0 + warp * 16) || (p.window_left >= 0);
+    const bool need_mask = (t0 + FA_BN > kv_end) || (p.causal && t0 + FA_BN - 1 > off + q0 + warp * 16) || (p.window_left >= 0);
     float mx[2] = {m_run[0], m_run[1]};
 #pragma unroll
     for (int j = 0; j < FA_BN / 8; j++) {
@@ -144,8 +160,8 @@ __global__ void __launch_bounds__(FA_THREADS, 1) prefill_attn_kernel(const FaPar
         else s *= p.scale_log2;
         if (need_mask) {
           const int col = t0 + 8 * j + 2 * (lane & 3) + (e & 1);
-          const int row = row_a + ((e >> 1) << 3);
-          const bool ok = col < len && (!p.causal || col <= row) && (p.window_left < 0 || col >= row - p.window_left);
+          const int pos = off + row_a + ((e >> 1) << 3);
+          const bool ok = col < kv_len && (!p.causal || col <= pos) && (p.window_left < 0 || col >= pos - p.window_left);
           if (!ok) s = -INFINITY;
         }
         sacc[j][e] = s;
@@ -212,9 +228,9 @@ __global__ void __launch_bounds__(FA_THREADS, 1) prefill_attn_kernel(const FaPar
   }
 }
 
-template <typename T, int D>
+template <typename T, int D, bool PAGED = false>
 static cudaError_t launch_fa(const FaParams &p, int batch, int max_len, cudaStream_t st) {
-  auto kern = prefill_attn_kernel<T, D>;
+  auto kern = prefill_attn_kernel<T, D, PAGED>;
   const size_t smem = 4 * (size_t)FA_BN * D * 2;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   dim3 grid((max_len + FA_BM - 1) / FA_BM, p.H, batch);
@@ -263,4 +279,46 @@ extern "C" int32_t mrs_prefill_attention(const void *q, const void *k, const voi
   if (head_dim == 128) return (int32_t)(dtype == 0 ? launch_fa<__half, 128>(p, nb, ml, st) : launch_fa<__nv_bfloat16, 128>(p, nb, ml, st));
   if (head_dim == 64) return (int32_t)(dtype == 0 ? launch_fa<__half, 64>(p, nb, ml, st) : launch_fa<__nv_bfloat16, 64>(p, nb, ml, st));
   return (int32_t)cudaErrorInvalidValue;
+}
+
+extern "C" int32_t mrs_prefill_attention_paged_tc(const void *q, const void *key_cache, const void *value_cache, void *out,
+                                                  const int32_t *block_table, int32_t block_table_stride,
+                                                  const int32_t *cu_seqlens_q, const int32_t *cu_seqlens_k, int32_t batch,
+                                                  int32_t total_q, int32_t max_seqlen_q, int32_t max_seqlen_k, int32_t num_blocks,
+                                                  int32_t num_heads, int32_t num_kv_heads, int32_t head_dim, int32_t page_size,
+                                                  int64_t q_stride, int64_t o_stride, float softmax_scale, int32_t causal,
+                                                  int32_t window_left, float softcap, uint32_t dtype, void *stream);   // prefill_attn_tc.cu
+
+// prompt attention of new query tokens over K/V already in the HND page cache; contract in include/mrs_b200_paged_attn.h
+extern "C" int32_t mrs_prefill_attention_paged(const void *q, const void *key_cache, const void *value_cache, void *out,
+                                               const int32_t *block_table, int32_t block_table_stride,
+                                               const int32_t *cu_seqlens_q, const int32_t *cu_seqlens_k, int32_t batch,
+                                               int32_t total_q, int32_t max_seqlen_q, int32_t max_seqlen_k, int32_t num_blocks,
+                                               int32_t num_heads, int32_t num_kv_heads, int32_t head_dim, int32_t page_size,
+                                               int64_t q_stride, int64_t o_stride, float softmax_scale, int32_t causal,
+                                               int32_t window_left, float softcap, uint32_t dtype, void *stream) {
+  if (total_q <= 0 || batch <= 0) return 0;
+  if ((dtype != 0 && dtype != 1) || (head_dim != 64 && head_dim != 128) || num_kv_heads <= 0 || num_heads % num_kv_heads ||
+      (page_size != 8 && page_size != 16 && page_size != 32) || (q_stride | o_stride) % 8 || num_blocks <= 0 ||
+      block_table == nullptr || cu_seqlens_q == nullptr || cu_seqlens_k == nullptr || block_table_stride <= 0)
+    return (int32_t)cudaErrorInvalidValue;
+  if (((uintptr_t)q | (uintptr_t)key_cache | (uintptr_t)value_cache | (uintptr_t)out) & 15) return (int32_t)cudaErrorMisalignedAddress;
+  {   // the wgmma kernel when the call fits it (head size 128, no window, no softcap)
+    const int32_t e = mrs_prefill_attention_paged_tc(q, key_cache, value_cache, out, block_table, block_table_stride, cu_seqlens_q,
+                                                     cu_seqlens_k, batch, total_q, max_seqlen_q, max_seqlen_k, num_blocks, num_heads,
+                                                     num_kv_heads, head_dim, page_size, q_stride, o_stride, softmax_scale, causal,
+                                                     window_left, softcap, dtype, stream);
+    if (e != (int32_t)cudaErrorNotSupported) return e;
+  }
+  FaParams p = {};
+  p.q = q; p.k = key_cache; p.v = value_cache; p.o = out; p.cu_seqlens = cu_seqlens_q; p.cu_seqlens_k = cu_seqlens_k;
+  p.block_table = block_table; p.bt_stride = block_table_stride; p.page_shift = page_size == 8 ? 3 : page_size == 16 ? 4 : 5;
+  p.T = total_q; p.H = num_heads; p.KVH = num_kv_heads;
+  p.q_stride = q_stride; p.kv_stride = head_dim; p.o_stride = o_stride;
+  p.softmax_scale = softmax_scale; p.scale_log2 = softmax_scale * 1.4426950408889634f;
+  p.softcap = softcap; p.causal = causal; p.window_left = window_left;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (head_dim == 128)
+    return (int32_t)(dtype == 0 ? launch_fa<__half, 128, true>(p, batch, max_seqlen_q, st) : launch_fa<__nv_bfloat16, 128, true>(p, batch, max_seqlen_q, st));
+  return (int32_t)(dtype == 0 ? launch_fa<__half, 64, true>(p, batch, max_seqlen_q, st) : launch_fa<__nv_bfloat16, 64, true>(p, batch, max_seqlen_q, st));
 }

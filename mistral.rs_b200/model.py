@@ -657,7 +657,9 @@ class LlamaPrefill:
     RMSNorm -> wgmma dequant-GEMMs (`mmq.forward`, the `fast_mmq` path) -> RoPE -> causal prompt
     attention over the fresh q/k/v (`paged_attn.prefill_attention`, the reference's flash-attn call,
     paged_attention.rs:1413-1475) -> KV scatter into the paged HND cache -> o_proj -> add+RMSNorm ->
-    GLU -> down -> add.  TTFT of BASELINE config 3 is the time of `forward` on a 4096-token prompt."""
+    GLU -> down -> add.  TTFT of BASELINE config 3 is the time of `forward` on a 4096-token prompt.
+    `forward(cached=n)` continues a sequence whose first n tokens are already in the cache (prefix-cache hit or
+    chunked prefill): KV scatter first, then paged prompt attention over the cache (`prefill_attention_paged`)."""
 
     def __init__(self, weights: "LlamaWeights", max_tokens=4096, runner: "LlamaRunner" = None):
         """runner: write the prompt's K/V into sequence 0 of this decode runner's paged cache (its block
@@ -681,16 +683,38 @@ class LlamaPrefill:
             self.v_cache = [torch.zeros(nb, cfg.n_kv_heads, bs, cfg.head_dim, dtype=dt, device=dev) for _ in range(cfg.n_layers)]
         self._slots = torch.tensor([self.table[i // bs] * bs + i % bs for i in range(self.max_tokens)], dtype=torch.int64, device=dev)
 
-    def forward(self, tokens, all_logits=False):
-        """tokens: list[int] (1 < len <= max_tokens).  Returns logits [vocab] of the last token, or
-        [T, vocab] with all_logits=True.  The KV cache of every layer holds rows 0..T-1 afterwards."""
+    def forward(self, tokens, all_logits=False, cached=0, table=None):
+        """tokens: list[int] (1 < len <= max_tokens), the prompt at positions cached .. cached + T - 1.  Returns logits
+        [vocab] of the last token, or [T, vocab] with all_logits=True.  The KV cache of every layer holds rows
+        cached .. cached + T - 1 afterwards.
+        cached > 0: rows 0 .. cached - 1 are already in the cache under `table` (a prefix-cache hit, or the earlier
+        chunks of a chunked prompt); only `tokens` are computed, and they attend to all cached + T keys through the
+        paged prefill kernel.  Then T == 1 is allowed.  table: block ids of the sequence (e.g.
+        `KVCacheManager.get_block_ids`), default the prefill's own table or the runner's."""
         from . import mmq, ops, paged_attn, quant
         cfg, dev, dt, w = self.cfg, self.dev, self.dt, self.w
-        T = len(tokens)
-        if not 1 < T <= min(self.max_tokens, cfg.max_pos):
-            raise ValueError(f"LlamaPrefill.forward: need 1 < tokens <= {min(self.max_tokens, cfg.max_pos)}, got {T}")
+        T, cached = len(tokens), int(cached)
+        bs = cfg.block_size
+        if cached == 0 and table is None:
+            if not 1 < T <= min(self.max_tokens, cfg.max_pos):
+                raise ValueError(f"LlamaPrefill.forward: need 1 < tokens <= {min(self.max_tokens, cfg.max_pos)}, got {T}")
+            slots = self._slots[:T]
+        else:
+            table = self.table if table is None else [int(b) for b in table]
+            end = cached + T
+            if cached < 0 or not (1 if cached else 2) <= T <= self.max_tokens:
+                raise ValueError(f"LlamaPrefill.forward: need cached >= 0 and {1 if cached else 2} <= tokens <= "
+                                 f"{self.max_tokens}, got cached={cached}, {T} tokens")
+            if end > min(cfg.max_pos, len(table) * bs):
+                raise ValueError(f"LlamaPrefill.forward: cached + tokens = {end} exceeds max_pos {cfg.max_pos} or the "
+                                 f"table's {len(table)} blocks of {bs}")
+            slots = torch.tensor([table[i // bs] * bs + i % bs for i in range(cached, end)], dtype=torch.int64, device=dev)
+            if cached:
+                positions = torch.arange(cached, end, dtype=torch.int32, device=dev)
+                block_table = torch.tensor([table], dtype=torch.int32, device=dev)
+                cu_q = torch.tensor([0, T], dtype=torch.int32, device=dev)
+                cu_k = torch.tensor([0, end], dtype=torch.int32, device=dev)
         H, KVH, D = cfg.n_heads, cfg.n_kv_heads, cfg.head_dim
-        slots = self._slots[:T]
         if torch.is_tensor(tokens):      # e.g. pinned host ids: the H2D copy is part of the call
             ids = tokens.to(device=dev, dtype=torch.int32, non_blocking=True)
         else:
@@ -710,9 +734,15 @@ class LlamaPrefill:
             q = mmq.forward(qt(L["attn_q"]), h).view(T, H, D)
             k = mmq.forward(qt(L["attn_k"]), h).view(T, KVH, D)
             v = mmq.forward(qt(L["attn_v"]), h).view(T, KVH, D)
-            ops.apply_rotary_qk(q, k, w.rope_cos, w.rope_sin, None, is_neox=cfg.rope_neox)
-            attn = paged_attn.prefill_attention(q, k, v, scale)
-            paged_attn.reshape_and_cache_flashinfer(k, v, self.k_cache[l], self.v_cache[l], slots)
+            if cached:   # the suffix's K/V go into the cache first, then attend over the whole sequence there
+                ops.apply_rotary_qk(q, k, w.rope_cos, w.rope_sin, positions, is_neox=cfg.rope_neox)
+                paged_attn.reshape_and_cache_flashinfer(k, v, self.k_cache[l], self.v_cache[l], slots)
+                attn = paged_attn.prefill_attention_paged(q, self.k_cache[l], self.v_cache[l], block_table, cu_q, cu_k,
+                                                          T, end, scale)
+            else:
+                ops.apply_rotary_qk(q, k, w.rope_cos, w.rope_sin, None, is_neox=cfg.rope_neox)
+                attn = paged_attn.prefill_attention(q, k, v, scale)
+                paged_attn.reshape_and_cache_flashinfer(k, v, self.k_cache[l], self.v_cache[l], slots)
             o = mmq.forward(qt(L["attn_output"]), attn.view(T, H * D))
             x, h2 = ops.add_rms_norm(o, x, L["ffn_norm"], cfg.rms_eps)       # x = o + x ; h2 = norm(x)
             gate = mmq.forward(qt(L["ffn_gate"]), h2)

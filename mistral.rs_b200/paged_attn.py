@@ -308,3 +308,54 @@ def prefill_attention(q, k, v, softmax_scale, causal=True, cu_seqlens=None, max_
     if rc != 0:
         raise RuntimeError(f"mrs_prefill_attention failed with cudaError {rc}")
     return out
+
+
+PREFILL_PAGE_SIZES = (8, 16, 32)   # the reference's allowed block sizes
+
+
+def prefill_attention_paged(q, key_cache, value_cache, block_table, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k,
+                            softmax_scale, causal=True, window_left=None, softcap=None):
+    """Prompt attention of new query tokens over K/V already in the HND page cache (the reference's
+    `flash_attn_varlen_paged_windowed`, paged_attention.rs:1357-1411): prefix-cache hits and chunked prompts.
+    q [total_q, H, D] (heads dense); key_cache / value_cache [num_blocks, KVH, page, D] in q's dtype, holding the new
+    tokens' K/V already; block_table [batch, max_pages] i32; cu_seqlens_q / cu_seqlens_k [batch + 1] i32, cumulative.
+    Query i of sequence b sits at position kv_len_b - q_len_b + i (causal mask aligned bottom-right) -> out [total_q, H, D]."""
+    if q.dtype not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"prefill_attention_paged: unsupported dtype {q.dtype}")
+    if key_cache.dtype != q.dtype or value_cache.dtype != q.dtype:
+        raise ValueError(f"prefill_attention_paged: cache dtype {key_cache.dtype}/{value_cache.dtype} must equal q's {q.dtype}")
+    if q.dim() != 3 or q.stride(2) != 1 or q.stride(1) != q.shape[2]:
+        raise ValueError("prefill_attention_paged: q must be [tokens, heads, head_dim] with dense heads")
+    T, H, D = q.shape
+    if key_cache.dim() != 4 or value_cache.shape != key_cache.shape or not (key_cache.is_contiguous() and value_cache.is_contiguous()):
+        raise ValueError("prefill_attention_paged: caches must be contiguous [num_blocks, kv_heads, page, head_dim] of one shape")
+    nb, KVH, page, d = key_cache.shape
+    if D not in (64, 128) or d != D:
+        raise ValueError(f"prefill_attention_paged: head_dim must be 64 or 128 and match the cache, got {D} / {d}")
+    if page not in PREFILL_PAGE_SIZES:
+        raise ValueError(f"prefill_attention_paged: page size must be one of {PREFILL_PAGE_SIZES}, got {page}")
+    if KVH == 0 or H % KVH:
+        raise ValueError(f"prefill_attention_paged: {H} query heads do not divide into {KVH} KV heads")
+    if block_table.dtype != torch.int32 or block_table.dim() != 2 or block_table.stride(1) != 1:
+        raise ValueError("prefill_attention_paged: block_table must be a 2-D i32 tensor with contiguous rows")
+    batch = cu_seqlens_q.numel() - 1
+    for name, t in (("cu_seqlens_q", cu_seqlens_q), ("cu_seqlens_k", cu_seqlens_k)):
+        if t.dtype != torch.int32 or t.dim() != 1 or t.numel() != batch + 1 or not t.is_contiguous():
+            raise ValueError(f"prefill_attention_paged: {name} must be a contiguous i32 vector of batch + 1 entries")
+    if block_table.shape[0] != batch:
+        raise ValueError(f"prefill_attention_paged: block_table has {block_table.shape[0]} rows for {batch} sequences")
+    if max_seqlen_k > block_table.shape[1] * page:
+        raise ValueError("prefill_attention_paged: max_seqlen_k exceeds the block table's capacity")
+    out = torch.empty(T, H, D, dtype=q.dtype, device=q.device)
+    rc = lib().mrs_prefill_attention_paged(_p(q), _p(key_cache), _p(value_cache), _p(out), _p(block_table),
+                                           ctypes.c_int(block_table.stride(0)), _p(cu_seqlens_q), _p(cu_seqlens_k),
+                                           ctypes.c_int(batch), ctypes.c_int(T), ctypes.c_int(int(max_seqlen_q)),
+                                           ctypes.c_int(int(max_seqlen_k)), ctypes.c_int(nb), ctypes.c_int(H), ctypes.c_int(KVH),
+                                           ctypes.c_int(D), ctypes.c_int(page), ctypes.c_int64(q.stride(0)),
+                                           ctypes.c_int64(out.stride(0)), ctypes.c_float(softmax_scale), ctypes.c_int(int(causal)),
+                                           ctypes.c_int(-1 if window_left is None else int(window_left)),
+                                           ctypes.c_float(0.0 if softcap is None else float(softcap)),
+                                           ctypes.c_uint32(_DT_CODE[q.dtype]), _stream(q.device))
+    if rc != 0:
+        raise RuntimeError(f"mrs_prefill_attention_paged failed with cudaError {rc}")
+    return out
