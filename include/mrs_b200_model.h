@@ -95,6 +95,40 @@ int32_t mrs_decode_advance(const int32_t *block_tables, int32_t max_blocks_per_s
                            int32_t *o_indptr, int32_t *kv_chunk_size, uint8_t *block_valid_mask,
                            int32_t max_pos, int32_t *error_flag, void *stream);
 
+/* Speculative decoding (REF mistralrs-core/src/speculative/, greedy verification): one verify step scores q_len =
+ * k + 1 rows per sequence — the anchor (the last sampled token, not yet in the cache) and k drafts — in one pass over
+ * the weights, then accepts drafts on the device.
+ *
+ * mrs_decode_advance_multi: mrs_decode_advance for q_len rows per sequence.  Sequence b at context c gets
+ * positions[b*q_len + i] = c + i with their slots, context_lens[b] = c + q_len, and the CSR / tile plan for that
+ * length.  A sequence with c + q_len > min(max_blocks_per_seq*block_size, max_pos) is frozen whole: all its slots are
+ * -1, context_lens[b] stays c, bit 0 of *error_flag is set.  q_len 1..8, that bound >= q_len.
+ *
+ * mrs_spec_accept: per sequence b, rows token_ids[b*q_len ..] = [anchor, draft 1..k] and argmax[b*q_len + i] = the
+ * target's token after row i.  a = number of leading i < k with draft i+1 == argmax[i]; emitted[b*q_len + i] =
+ * argmax[b*q_len + i] for i <= a, else -1; accepted[b] = a; context_lens[b] goes from c + q_len to c + 1 + a; the next
+ * anchor token_ids[b*q_len] = argmax[b*q_len + a].  A frozen sequence (slot_mapping[b*q_len] < 0) gets accepted -1,
+ * emitted all -1 and keeps its context and anchor.
+ *
+ * mrs_llama_verify_step: s->batch = B sequences, every row buffer of `s` (token_ids, positions, slot_mapping, x, x2,
+ * q, k, v, attn_out, act, logits, out_token) holds B*q_len rows, tmp_v / tmp_s hold [padded_tiles, q_len*n_heads],
+ * attn_counters B*n_kv_heads*ceil(group*q_len/16), argmax_scratch >= 16*B*q_len + 16 bytes; the metadata comes from
+ * mrs_decode_advance_multi.  Embedding gather of the B*q_len ids -> the decode layer chain with the multi-query fused
+ * attention -> lm_head on every row -> mrs_argmax into out_token (must not alias token_ids) -> mrs_spec_accept with
+ * `context_lens` (the lengths the advance read; the step struct carries none).  Graph-capturable.  skip_mask as for
+ * decode.  cudaErrorInvalidValue for B*q_len > 8, q_len outside 2..8, fused_attention == 0, head_dim other than 64 /
+ * 128, or tp / all_reduce set. */
+int32_t mrs_decode_advance_multi(const int32_t *block_tables, int32_t max_blocks_per_seq, int32_t *context_lens,
+                                 int32_t batch, int32_t block_size, int32_t split_pages, int32_t padded_tiles,
+                                 int32_t *positions, int64_t *slot_mapping, int32_t *kv_indptr, int32_t *kv_indices,
+                                 int32_t *kv_last_page_len, int32_t *request_indices, int32_t *kv_tile_indices,
+                                 int32_t *o_indptr, int32_t *kv_chunk_size, uint8_t *block_valid_mask,
+                                 int32_t max_pos, int32_t *error_flag, int32_t q_len, void *stream);
+int32_t mrs_spec_accept(const int32_t *argmax, int32_t *token_ids, const int64_t *slot_mapping, int32_t *context_lens,
+                        int32_t *accepted, int32_t *emitted, int32_t batch, int32_t q_len, int32_t pdl, void *stream);
+int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,
+                              int32_t *emitted, void *stream);
+
 /* rows of a quantised table -> activation dtype (embedding gather). ids on device. */
 int32_t mrs_embedding_gather(int32_t ggml_type, const void *table, int32_t cols, const int32_t *ids, int32_t n,
                              void *out, int32_t act_dtype, void *stream);

@@ -107,6 +107,24 @@ int32_t mrs_paged_decode_fused_strided(void *q, void *k_new, void *v_new, void *
                                int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size, int32_t page_size,
                                float sm_scale, uint32_t dtype, int32_t pdl, int64_t q_stride_n, int64_t kv_new_stride,
                                void *stream);
+/* Multi-query form (speculative verify): every sequence brings q_len rows (1..8) at positions kv_len - q_len ..
+ * kv_len - 1, where kv_len (from the CSR) already counts them.  q / k_new / v_new / o / positions / slot_mapping hold
+ * [batch_size * q_len] rows, sequence-major; q and o are contiguous [*, num_qo_heads * head_size], k_new / v_new
+ * [*, num_kv_heads * head_size].  Query row i attends to every cached row below kv_len - q_len and to new rows 0..i
+ * (causal); the new rows are rotated, attended from shared memory and written to their slots (slot < 0: not
+ * written).  No cached row at or past kv_len - q_len is read.  tmp_v / tmp_s: [padded_batch_size, q_len *
+ * num_qo_heads] partials; counters: zeroed int32 [batch_size * num_kv_heads * ceil(group * q_len / 16)], left zero.
+ * Head size 64 | 128, dtype 0 f16 / 1 bf16, no window / soft-cap.  At q_len = 1 the result equals
+ * mrs_paged_decode_fused bit for bit.  Returns a cudaError_t. */
+int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
+                               const void *rope_cos, const void *rope_sin, const int32_t *positions,
+                               const int64_t *slot_mapping, const int32_t *kv_indptr, const int32_t *kv_indices,
+                               const int32_t *kv_last_page_len, const int32_t *request_indices,
+                               const int32_t *kv_tile_indices, const int32_t *o_indptr,
+                               const int32_t *kv_chunk_size_ptr, const uint8_t *block_valid_mask, void *o, void *tmp_v,
+                               float *tmp_s, int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
+                               int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size, int32_t page_size,
+                               float sm_scale, uint32_t dtype, int32_t pdl, int32_t q_len, void *stream);
 /* ---- prompt attention over fresh q/k/v (SURVEY §8(f) rank 1; REF paged_attention.rs:1413-1475 ->
  * flash_attn_varlen): causal [+ sliding window / soft-cap], GQA, var-len batches via cu_seqlens
  * (device i32 [batch+1], or NULL for one sequence).  q [total,H,D], k/v [total,KVH,D], strides in

@@ -1,6 +1,7 @@
 // decoder.cu — the caller of the hot path: a Llama-family decode layer stack over the kernels in
 // this library (see include/mrs_b200_model.h), plus the few glue kernels a token step needs
-// (quantised embedding gather, argmax, on-device KV index advance).
+// (quantised embedding gather, argmax, on-device KV index advance, greedy acceptance of a speculative
+// verify step).
 //
 // REF structure being mirrored: mistralrs-core/src/models/llama.rs:68-135 (attention),
 // :243-260 (block), :475-… (model forward); embedding gather over ggml blocks:
@@ -38,6 +39,17 @@ extern "C" int32_t mrs_paged_decode_fused(void *q, void *k_new, void *v_new, voi
                                           int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
                                           int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
                                           void *stream);
+extern "C" int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
+                                                const void *rope_cos, const void *rope_sin, const int32_t *positions,
+                                                const int64_t *slot_mapping, const int32_t *kv_indptr,
+                                                const int32_t *kv_indices, const int32_t *kv_last_page_len,
+                                                const int32_t *request_indices, const int32_t *kv_tile_indices,
+                                                const int32_t *o_indptr, const int32_t *kv_chunk_size_ptr,
+                                                const uint8_t *block_valid_mask, void *o, void *tmp_v, float *tmp_s,
+                                                int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
+                                                int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
+                                                int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
+                                                int32_t q_len, void *stream);
 extern "C" int32_t flashinfer_decode(void *q, void *key_cache, void *value_cache, const int32_t *kv_indptr,
                                      const int32_t *kv_indices, const int32_t *kv_last_page_len,
                                      const int32_t *request_indices, const int32_t *kv_tile_indices,
@@ -233,23 +245,30 @@ __global__ void __launch_bounds__(1024) tp_allreduce_ll_kernel(const ArCtxDev c,
 // table (pos >= min(max_blocks*bs, max_pos)) is frozen: its context does not grow, its KV write is
 // skipped (slot -1, the reference's _PAD_SLOT_ID) and *error_flag gets bit 0 — generation past the
 // allocated context must never turn into an out-of-bounds cache write.
+// q > 1 (speculative verify): sequence b processes q rows at positions c .. c + q - 1 (rows b * q + i of positions /
+// slot_mapping) and its context becomes c + q.  A sequence with c + q > cap is frozen whole: every slot is -1 and its
+// context_lens entry keeps c (the acceptance kernel recognises it by slot -1 and leaves it there); its attention
+// still runs over the last q table positions, whose rows are never written.  Requires cap >= q.
 constexpr int ADV_MAX_BATCH = 256;
 __global__ void decode_advance_kernel(const int32_t *__restrict__ block_tables, int max_blocks,
                                       int32_t *__restrict__ context_lens, int batch, int bs, int split_pages,
                                       int padded_tiles, int max_pos, int32_t *positions, int64_t *slot_mapping,
                                       int32_t *kv_indptr, int32_t *kv_indices, int32_t *kv_last_page_len,
                                       int32_t *request_indices, int32_t *kv_tile_indices, int32_t *o_indptr,
-                                      int32_t *kv_chunk_size, uint8_t *block_valid_mask, int32_t *error_flag) {
+                                      int32_t *kv_chunk_size, uint8_t *block_valid_mask, int32_t *error_flag, int q) {
   __shared__ int s_nb[ADV_MAX_BATCH], s_chunks[ADV_MAX_BATCH], s_indptr[ADV_MAX_BATCH + 1], s_oind[ADV_MAX_BATCH + 1];
   const int cap = min(max_blocks * bs, max_pos > 0 ? max_pos : max_blocks * bs);
   for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-    int pos = context_lens[b];             // position of the token being processed now
-    const bool full = pos >= cap;
-    if (full) { pos = cap - 1; if (error_flag != nullptr) atomicOr(error_flag, 1); }
-    const int ctx = pos + 1;               // context length including it
-    context_lens[b] = ctx;
-    positions[b] = pos;
-    slot_mapping[b] = full ? (int64_t)-1 : (int64_t)block_tables[(int64_t)b * max_blocks + pos / bs] * bs + pos % bs;
+    const int c = context_lens[b];         // position of the (first) token being processed now
+    const bool full = c + q > cap;
+    if (full && error_flag != nullptr) atomicOr(error_flag, 1);
+    const int ctx = full ? cap : c + q;    // context length including the processed tokens
+    context_lens[b] = (full && q > 1) ? c : ctx;
+    for (int i = 0; i < q; i++) {
+      const int pos = ctx - q + i;
+      positions[b * q + i] = pos;
+      slot_mapping[b * q + i] = full ? (int64_t)-1 : (int64_t)block_tables[(int64_t)b * max_blocks + pos / bs] * bs + pos % bs;
+    }
     const int nb = (ctx + bs - 1) / bs;
     s_nb[b] = nb;
     kv_last_page_len[b] = ctx - (nb - 1) * bs;
@@ -280,6 +299,32 @@ __global__ void decode_advance_kernel(const int32_t *__restrict__ block_tables, 
     block_valid_mask[t] = t < tiles ? 1 : 0;
     if (t >= tiles) { request_indices[t] = 0; kv_tile_indices[t] = 0; }
   }
+}
+
+// greedy acceptance of a verify step (REF mistralrs-core/src/speculative/verifier.rs:198-291, top-1 rule): sequence b
+// fed rows [anchor, draft 1 .. k] (token_ids[b * q ..]) and argmax[b * q + i] is the target's choice after row i.
+// Drafts are accepted while draft i + 1 == argmax[i]; a accepted drafts emit argmax[0 .. a] (a + 1 tokens), the
+// context keeps the anchor and the accepted drafts (c + 1 + a, the reference's keep_len) and argmax[a] is the next
+// anchor.  A sequence the advance froze (slot -1) emits nothing: accepted -1, emitted all -1, context unchanged.
+__global__ void spec_accept_kernel(const int32_t *__restrict__ argmax, int32_t *__restrict__ token_ids,
+                                   const int64_t *__restrict__ slot_mapping, int32_t *__restrict__ context_lens,
+                                   int32_t *__restrict__ accepted, int32_t *__restrict__ emitted, int batch, int q, int pdl) {
+  if (pdl) pdl_wait();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  const int32_t *am = argmax + (int64_t)b * q;
+  int32_t *row = token_ids + (int64_t)b * q, *em = emitted + (int64_t)b * q;
+  if (slot_mapping[(int64_t)b * q] < 0) {
+    accepted[b] = -1;
+    for (int i = 0; i < q; i++) em[i] = -1;
+    return;
+  }
+  int a = 0;
+  while (a < q - 1 && row[a + 1] == am[a]) a++;
+  for (int i = 0; i < q; i++) em[i] = (i <= a) ? am[i] : -1;
+  accepted[b] = a;
+  context_lens[b] += 1 + a - q;            // the advance left c + q
+  row[0] = am[a];
 }
 
 }  // namespace mrs
@@ -322,8 +367,41 @@ extern "C" int32_t mrs_decode_advance(const int32_t *block_tables, int32_t max_b
                                                              block_size, split_pages, padded_tiles, max_pos, positions,
                                                              slot_mapping, kv_indptr, kv_indices, kv_last_page_len,
                                                              request_indices, kv_tile_indices, o_indptr, kv_chunk_size,
-                                                             block_valid_mask, error_flag);
+                                                             block_valid_mask, error_flag, 1);
   return (int32_t)cudaGetLastError();
+}
+
+extern "C" int32_t mrs_decode_advance_multi(const int32_t *block_tables, int32_t max_blocks_per_seq, int32_t *context_lens,
+                                            int32_t batch, int32_t block_size, int32_t split_pages, int32_t padded_tiles,
+                                            int32_t *positions, int64_t *slot_mapping, int32_t *kv_indptr,
+                                            int32_t *kv_indices, int32_t *kv_last_page_len, int32_t *request_indices,
+                                            int32_t *kv_tile_indices, int32_t *o_indptr, int32_t *kv_chunk_size,
+                                            uint8_t *block_valid_mask, int32_t max_pos, int32_t *error_flag, int32_t q_len,
+                                            void *stream) {
+  if (batch < 1 || batch > ADV_MAX_BATCH || max_blocks_per_seq < 1 || block_size < 1 || q_len < 1 || q_len > 8)
+    return (int32_t)cudaErrorInvalidValue;
+  const int cap = max_pos > 0 && max_pos < max_blocks_per_seq * block_size ? max_pos : max_blocks_per_seq * block_size;
+  if (cap < q_len) return (int32_t)cudaErrorInvalidValue;
+  decode_advance_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(block_tables, max_blocks_per_seq, context_lens, batch,
+                                                             block_size, split_pages, padded_tiles, max_pos, positions,
+                                                             slot_mapping, kv_indptr, kv_indices, kv_last_page_len,
+                                                             request_indices, kv_tile_indices, o_indptr, kv_chunk_size,
+                                                             block_valid_mask, error_flag, q_len);
+  return (int32_t)cudaGetLastError();
+}
+
+extern "C" int32_t mrs_spec_accept(const int32_t *argmax, int32_t *token_ids, const int64_t *slot_mapping,
+                                   int32_t *context_lens, int32_t *accepted, int32_t *emitted, int32_t batch, int32_t q_len,
+                                   int32_t pdl, void *stream) {
+  if (batch < 1 || q_len < 1) return (int32_t)cudaErrorInvalidValue;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((batch + 127) / 128); cfg.blockDim = dim3(128); cfg.stream = (cudaStream_t)stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+  return (int32_t)cudaLaunchKernelEx(&cfg, spec_accept_kernel, argmax, token_ids, slot_mapping, context_lens, accepted,
+                                     emitted, (int)batch, (int)q_len, (int)pdl);
 }
 
 extern "C" int32_t mrs_tp_allreduce_residual(const mrs_tp_ctx *ctx, int32_t slot, const void *residual, void *out,
@@ -374,11 +452,12 @@ extern "C" int32_t mrs_tp_allreduce_residual(const mrs_tp_ctx *ctx, int32_t slot
     }                                                  \
   } while (0)
 
-extern "C" int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream) {
-  const int dt = s->act_dtype, B = s->batch, H = s->hidden, pdl = s->pdl;
+// the layer stack + lm_head + argmax over batch * q_len token rows; q_len > 1 is a speculative verify step (every
+// sequence's rows attend through mrs_paged_decode_fused_multi), q_len == 1 the decode step
+static int32_t llama_forward(const mrs_llama_step *s, int q_len, void *stream) {
+  const int dt = s->act_dtype, NS = s->batch, B = s->batch * q_len, H = s->hidden, pdl = s->pdl;
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
   cudaStream_t st = (cudaStream_t)stream;
-  if (B < 1 || B > 8) return (int32_t)cudaErrorInvalidValue;
   const bool do_attn = !(s->skip_mask & 1), do_gemv = !(s->skip_mask & 2);
 
   MRS_TRY(mrs_embedding_gather(s->tok_embd.ggml_type, s->tok_embd.data, H, s->token_ids, B, s->x, dt, stream));
@@ -407,7 +486,15 @@ extern "C" int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream) 
       MRS_TRY(mrs_mmvq_fused(L.wv.ggml_type, 0, dt, L.wv.data, nullptr, nullptr, hidden, L.attn_norm, s->rms_eps,
                              nullptr, s->v, nullptr, nullptr, H, nkv, 0, 0, B, 0, pdl, stream));
     }
-    if (do_attn && s->fused_attention) {
+    if (do_attn && q_len > 1) {
+      MRS_TRY(mrs_paged_decode_fused_multi(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
+                                           s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
+                                           s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
+                                           s->block_valid_mask, s->attn_out, s->padded_tiles > NS ? s->tmp_v : nullptr,
+                                           s->padded_tiles > NS ? s->tmp_s : nullptr, s->attn_counters, NS, s->padded_tiles,
+                                           s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
+                                           pdl | (s->rope_neox ? 0 : 2), q_len, stream));
+    } else if (do_attn && s->fused_attention) {
       MRS_TRY(mrs_paged_decode_fused(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
                                      s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
                                      s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
@@ -469,4 +556,20 @@ extern "C" int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream) 
                          s->rms_eps, nullptr, s->logits, nullptr, nullptr, H, s->vocab, 0, 0, B, 0, pdl, stream));
   MRS_TRY(mrs_argmax(s->logits, B, s->vocab, dt, s->out_token, s->argmax_scratch, pdl, stream));
   return 0;
+}
+
+extern "C" int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream) {
+  if (s->batch < 1 || s->batch > 8) return (int32_t)cudaErrorInvalidValue;
+  return llama_forward(s, 1, stream);
+}
+
+extern "C" int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,
+                                         int32_t *emitted, void *stream) {
+  if (q_len < 2 || q_len > 8 || s->batch < 1 || s->batch * q_len > 8 || s->tp != nullptr || s->all_reduce != nullptr ||
+      !s->fused_attention || (s->head_dim != 64 && s->head_dim != 128) || s->out_token == s->token_ids ||
+      context_lens == nullptr || accepted == nullptr || emitted == nullptr)
+    return (int32_t)cudaErrorInvalidValue;
+  MRS_TRY(llama_forward(s, q_len, stream));
+  return mrs_spec_accept(s->out_token, s->token_ids, s->slot_mapping, context_lens, accepted, emitted, s->batch, q_len,
+                         s->pdl, stream);
 }

@@ -64,6 +64,7 @@ struct PagedParams {
   const int64_t *slot_mapping;
   const int32_t *o_indptr;
   int *counters;
+  int q_len;                // mrs_paged_decode_fused_multi: query rows per sequence (q, k_new, v_new, out: [B * q_len, ...])
 };
 
 template <typename T> struct Vec8;
@@ -614,6 +615,33 @@ static cudaError_t launch_pa(K kern, dim3 grid, const PagedParams &p, cudaStream
   return cudaLaunchKernelEx(&cfg, kern, p);
 }
 
+// the split tiles of one sequence as one thread-block cluster (merge through DSMEM).  Returns false, launching nothing,
+// when the device cannot schedule that cluster shape: asked once per shape through `feasible` (0 unknown, 1 yes,
+// -1 no), because a failed launch inside a stream capture would poison the capture
+template <typename K>
+static bool launch_pm_cluster(K kern, dim3 grid, const PagedParams &p, cudaStream_t st, size_t dyn, int *feasible, cudaError_t *err) {
+  const int tiles = (int)grid.x;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = dim3(PM_THREADS); cfg.dynamicSmemBytes = dyn; cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = tiles; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  if (feasible[tiles] == 0) {
+    int ncl = 0;
+    const cudaError_t qe = cudaOccupancyMaxActiveClusters(&ncl, kern, &cfg);
+    feasible[tiles] = (qe == cudaSuccess && ncl >= 1) ? 1 : -1;
+    if (qe != cudaSuccess) (void)cudaGetLastError();
+  }
+  if (feasible[tiles] != 1) return false;
+  cfg.numAttrs = p.pdl ? 2 : 1;
+  *err = cudaLaunchKernelEx(&cfg, kern, p);
+  return true;
+}
+
 template <typename T, typename CT, int D, int LAYOUT, bool FUSED>
 static cudaError_t launch_decode_g(PagedParams p, int tiles, cudaStream_t st) {
   const int group = p.num_heads / p.num_kv_heads;
@@ -627,30 +655,9 @@ static cudaError_t launch_decode_g(PagedParams p, int tiles, cudaStream_t st) {
         // one sequence split into <= 8 tiles: the tiles form a cluster and merge through DSMEM
         // (batch > 1 plans are compacted per sequence, so a fixed cluster size would straddle sequences)
         if (!(g_pa_flags & 2) && p.tmp_o != nullptr && p.batch_size == 1 && tiles <= PM_CL_MAX && nsub == 1 && p.heads_per_cta <= PM_CL_G) {
-          auto kern = paged_decode_mma_kernel<T, D, true, true>;
-          const size_t dyn = pm_smem_bytes<D>(true, true);
-          cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-          cudaLaunchConfig_t cfg = {};
-          cfg.gridDim = grid; cfg.blockDim = dim3(PM_THREADS); cfg.dynamicSmemBytes = dyn; cfg.stream = st;
-          cudaLaunchAttribute attr[2];
-          attr[0].id = cudaLaunchAttributeClusterDimension;
-          attr[0].val.clusterDim.x = tiles; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-          attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-          attr[1].val.programmaticStreamSerializationAllowed = 1;
-          cfg.attrs = attr; cfg.numAttrs = 1;
-          // is this cluster shape schedulable on the device?  (asked once per shape; a failed launch inside a
-          // stream capture would poison the capture, so never find out by trying)
-          static int feasible[PM_CL_MAX + 1] = {};   // 0 unknown, 1 yes, -1 no
-          if (feasible[tiles] == 0) {
-            int ncl = 0;
-            const cudaError_t qe = cudaOccupancyMaxActiveClusters(&ncl, kern, &cfg);
-            feasible[tiles] = (qe == cudaSuccess && ncl >= 1) ? 1 : -1;
-            if (qe != cudaSuccess) (void)cudaGetLastError();
-          }
-          if (feasible[tiles] == 1) {
-            cfg.numAttrs = p.pdl ? 2 : 1;
-            return cudaLaunchKernelEx(&cfg, kern, p);
-          }
+          static int feasible[PM_CL_MAX + 1] = {};
+          cudaError_t e;
+          if (launch_pm_cluster(paged_decode_mma_kernel<T, D, true, true>, grid, p, st, pm_smem_bytes<D>(true, true), feasible, &e)) return e;
         }
       }
       return launch_pa(paged_decode_mma_kernel<T, D, FUSED, false>, grid, p, st, pm_smem_bytes<D>(FUSED, false), PM_THREADS);
@@ -672,6 +679,24 @@ static cudaError_t launch_decode_g(PagedParams p, int tiles, cudaStream_t st) {
   }
   if constexpr (D <= 128) return launch_pa(paged_decode_kernel<T, CT, D, 8, LAYOUT, FUSED>, grid, p, st, dyn);
   return cudaErrorInvalidValue;
+}
+
+// multi-query fused decode: the MMA rows of a KV head are its group x q_len (query, head) pairs, in slices of <= 16
+// over blockIdx.z.  The cluster merge buffer holds a whole 16-row slice (PM_CL_GM), so every one-slice batch-1 split
+// plan merges through DSMEM; larger shapes merge through the counter.
+template <typename T, int D>
+static cudaError_t launch_decode_multi(PagedParams p, int tiles, cudaStream_t st) {
+  if (tiles <= 0) return cudaSuccess;
+  const int rows = p.num_heads / p.num_kv_heads * p.q_len;
+  const int nsub = (rows + 15) / 16;
+  p.heads_per_cta = (rows + nsub - 1) / nsub;
+  dim3 grid(tiles, p.num_kv_heads, nsub);
+  if (!(g_pa_flags & 2) && p.tmp_o != nullptr && p.batch_size == 1 && tiles <= PM_CL_MAX && nsub == 1) {
+    static int feasible[PM_CL_MAX + 1] = {};
+    cudaError_t e;
+    if (launch_pm_cluster(paged_decode_mma_multi_kernel<T, D, true>, grid, p, st, pm_smem_bytes<D>(true, true, PM_CL_GM), feasible, &e)) return e;
+  }
+  return launch_pa(paged_decode_mma_multi_kernel<T, D, false>, grid, p, st, pm_smem_bytes<D>(true, false), PM_THREADS);
 }
 
 // head sizes: REF pagedattention.cuh:718-739 (64, 80, 96, 112, 128, 192, 256) + 512 (flashinfer/mod.rs:262)
@@ -921,6 +946,51 @@ extern "C" int32_t mrs_paged_decode_fused(void *q, void *k_new, void *v_new, voi
                                         kv_chunk_size_ptr, block_valid_mask, o, tmp_v, tmp_s, counters, batch_size,
                                         padded_batch_size, num_qo_heads, num_kv_heads, head_size, page_size, sm_scale, dtype,
                                         pdl, (int64_t)num_qo_heads * head_size, (int64_t)num_kv_heads * head_size, stream);
+}
+
+// Multi-query form of mrs_paged_decode_fused (speculative verify): q_len rows per sequence at positions
+// kv_len - q_len .. kv_len - 1, laid out [B * q_len, ...] in q / k_new / v_new / positions / slot_mapping / o;
+// partials tmp_v / tmp_s [padded_batch_size, q_len * num_qo_heads]; counters [B * KVH * ceil(group * q_len / 16)].
+// Head size 64 | 128, q_len 1..8, 16-bit dtypes.  A sequence needs kv_len >= q_len.
+extern "C" int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
+                                                const void *rope_cos, const void *rope_sin, const int32_t *positions,
+                                                const int64_t *slot_mapping, const int32_t *kv_indptr,
+                                                const int32_t *kv_indices, const int32_t *kv_last_page_len,
+                                                const int32_t *request_indices, const int32_t *kv_tile_indices,
+                                                const int32_t *o_indptr, const int32_t *kv_chunk_size_ptr,
+                                                const uint8_t *block_valid_mask, void *o, void *tmp_v, float *tmp_s,
+                                                int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
+                                                int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
+                                                int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
+                                                int32_t q_len, void *stream) {
+  if ((dtype != 0 && dtype != 1) || (head_size != 64 && head_size != 128) || q_len < 1 || q_len > 8 || num_kv_heads < 1 ||
+      num_qo_heads % num_kv_heads)
+    return (int32_t)cudaErrorInvalidValue;
+  PagedParams p = {};
+  p.q = q; p.kc = key_cache; p.vc = value_cache; p.out = o;
+  const bool split = tmp_v != nullptr && padded_batch_size > batch_size;
+  p.tmp_o = split ? tmp_v : nullptr; p.tmp_lse = split ? tmp_s : nullptr;
+  if (split) {
+    p.request_indices = request_indices; p.kv_tile_indices = kv_tile_indices;
+    p.block_valid_mask = block_valid_mask; p.kv_chunk_size_ptr = kv_chunk_size_ptr;
+  }
+  p.kv_indptr = kv_indptr; p.kv_indices = kv_indices; p.kv_last_page_len = kv_last_page_len;
+  p.kv_block_stride = (int64_t)num_kv_heads * page_size * head_size; p.kv_head_stride = (int64_t)page_size * head_size;
+  p.num_heads = num_qo_heads; p.num_kv_heads = num_kv_heads; p.page_size = page_size;
+  p.q_stride_n = (int64_t)num_qo_heads * head_size; p.q_stride_h = head_size; p.sm_scale = sm_scale;
+  p.window_left = -1; p.pdl = pdl & 1; p.rope_interleaved = (pdl >> 1) & 1;
+  p.k_new = k_new; p.v_new = v_new; p.kv_new_stride = (int64_t)num_kv_heads * head_size;
+  p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.positions = positions; p.slot_mapping = slot_mapping;
+  p.o_indptr = o_indptr; p.counters = counters; p.batch_size = batch_size;
+  p.k_scale = 1.f; p.v_scale = 1.f;
+  p.q_len = q_len;
+  const int tiles = split ? padded_batch_size : batch_size;
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e;
+  if (dtype == 0) e = head_size == 64 ? launch_decode_multi<__half, 64>(p, tiles, st) : launch_decode_multi<__half, 128>(p, tiles, st);
+  else e = head_size == 64 ? launch_decode_multi<__nv_bfloat16, 64>(p, tiles, st) : launch_decode_multi<__nv_bfloat16, 128>(p, tiles, st);
+  if (e != cudaSuccess) fprintf(stderr, "mrs_b200: mrs_paged_decode_fused_multi failed: %s\n", cudaGetErrorString(e));
+  return (int32_t)e;
 }
 
 // bit 0: keep HND decode attention on the SIMT kernel instead of the tensor-core one; bit 1: no cluster/DSMEM

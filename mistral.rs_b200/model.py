@@ -753,3 +753,190 @@ class LlamaPrefill:
         if all_logits:
             return mmq.forward(qt(w.output), h)
         return quant.plain(qt(w.output), h[T - 1:T].contiguous())[0]
+
+
+def check_drafts(drafts, batch, draft_len, vocab):
+    """drafts as int32 [batch, draft_len] (a [B][k] list or a CPU tensor); ValueError on a wrong shape or an id outside
+    the vocabulary."""
+    t = drafts if torch.is_tensor(drafts) else torch.as_tensor(np.asarray(drafts, dtype=np.int64))
+    if t.device.type != "cpu" or tuple(t.shape) != (batch, draft_len):
+        raise ValueError(f"drafts must be a host [{batch}][{draft_len}] array, got {tuple(t.shape)} on {t.device}")
+    if t.dtype.is_floating_point or t.dtype == torch.bool:
+        raise ValueError(f"draft ids must be integers, got {t.dtype}")
+    if t.numel() and (int(t.min()) < 0 or int(t.max()) >= vocab):
+        raise ValueError(f"draft ids must lie in [0, {vocab})")
+    return t if t.dtype == torch.int32 else t.to(torch.int32)
+
+
+def check_verifier_args(runner, draft_len):
+    """ValueError unless `runner` can run verify steps of `draft_len` drafts (see LlamaVerifier)."""
+    k = int(draft_len)
+    if not 1 <= k <= 7:
+        raise ValueError(f"draft_len must be 1..7, got {draft_len}")
+    if runner.B * (k + 1) > 8:
+        raise ValueError(f"batch x (draft_len + 1) = {runner.B} x {k + 1} exceeds the 8 rows of one verify step")
+    if runner.w.tp_size != 1 or runner._peer is not None or runner._ar_cb is not None:
+        raise ValueError("speculative verification runs single-GPU (no tensor parallelism)")
+    if runner.cfg.head_dim not in (64, 128):
+        raise ValueError(f"verify attention supports head_dim 64 / 128, got {runner.cfg.head_dim}")
+    if runner.dt not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"verify steps run in f16 / bf16, got {runner.dt}")
+    if not runner.step_struct.fused_attention:
+        raise ValueError("verify steps need the runner's fused attention path")
+    if runner.max_ctx < k + 1:
+        raise ValueError(f"the runner's context ({runner.max_ctx}) is shorter than one verify step ({k + 1} rows)")
+    return k
+
+
+class LlamaVerifier:
+    """Greedy speculative decoding on a LlamaRunner's sequences (REF mistralrs-core/src/speculative/): each verify step
+    feeds q = k + 1 rows per sequence — the anchor (the token the runner would process next) and k caller-proposed
+    drafts — through mrs_llama_verify_step in one pass over the weights, and accepts drafts on the device
+    (mrs_spec_accept).
+
+    Shares the runner's weights, KV caches, block tables, context_lens and error_flag, so verify steps and plain
+    `runner.step()` calls can be mixed; owns the B*q-row metadata and scratch.  The anchor moves explicitly:
+    `sync_from_runner()` takes it from runner.meta["token_ids"], `sync_to_runner()` hands the next one back.  Rows a
+    step rejected stay in the cache past the context and are overwritten later (never read)."""
+
+    def __init__(self, runner: LlamaRunner, draft_len: int):
+        k = check_verifier_args(runner, draft_len)
+        r, cfg, dev, dt = runner, runner.cfg, runner.dev, runner.dt
+        B, q = runner.B, k + 1
+        R = B * q
+        self.r, self.k, self.q, self.B, self.dev, self.vocab = runner, k, q, B, dev, cfg.vocab
+        z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=dev)
+        self.meta = dict(token_ids=z(R), positions=z(R), slot_mapping=z(R, d=torch.int64),
+                         kv_indptr=z(B + 1), kv_indices=z(B * r.max_blocks), kv_last_page_len=z(B),
+                         request_indices=z(r.padded_tiles), kv_tile_indices=z(r.padded_tiles),
+                         o_indptr=z(B + 1), kv_chunk_size=z(1), block_valid_mask=z(r.padded_tiles, d=torch.uint8))
+        a = lambda *s: torch.zeros(*s, dtype=dt, device=dev)
+        H, D, n_heads, n_kv = cfg.hidden, cfg.head_dim, r.n_heads, r.n_kv
+        nsub = -(-(n_heads // n_kv) * q // 16)
+        self.buf = dict(x=a(R, H), x2=a(R, H), q=a(R, n_heads * D), k=a(R, n_kv * D), v=a(R, n_kv * D),
+                        attn_out=a(R, n_heads * D), act=a(R, cfg.inter), logits=a(R, cfg.vocab),
+                        tmp_v=a(r.padded_tiles, q * n_heads, D),
+                        tmp_s=torch.zeros(r.padded_tiles, q * n_heads, dtype=torch.float32, device=dev),
+                        out_token=z(R), attn_counters=z(B * n_kv * nsub),
+                        argmax_scratch=torch.zeros(16 * R + 16, dtype=torch.uint8, device=dev))
+        self.results = z(B + R)                       # accepted [B] then emitted [B*q]: one D2H copy per step
+        self._results_h = torch.zeros(B + R, dtype=torch.int32).pin_memory()
+        self._drafts_h = torch.zeros(B, k, dtype=torch.int32).pin_memory()
+        self._h2d_done = torch.cuda.Event()
+        s = _Step.from_buffer_copy(runner.step_struct)   # weights, caches, shapes, pdl: the runner's
+        for n, t in self.meta.items():
+            setattr(s, n, t.data_ptr())
+        for n, t in self.buf.items():
+            setattr(s, n, t.data_ptr())
+        self.step_struct = s
+        self.graph = None
+
+    def sync_from_runner(self):
+        """anchor of every sequence <- runner.meta["token_ids"]"""
+        self.meta["token_ids"].view(self.B, self.q)[:, 0].copy_(self.r.meta["token_ids"])
+
+    def sync_to_runner(self):
+        """runner.meta["token_ids"] <- the anchor the last verify step left (the token to process next)"""
+        self.r.meta["token_ids"].copy_(self.meta["token_ids"].view(self.B, self.q)[:, 0])
+
+    def set_drafts(self, drafts):
+        """drafts: [B][k] ids (list or host tensor) -> rows 1..k of every sequence (one pinned H2D copy)."""
+        t = check_drafts(drafts, self.B, self.k, self.vocab)
+        if not t.is_pinned():
+            self._h2d_done.synchronize()              # the previous copy out of the staging buffer has finished
+            self._drafts_h.copy_(t)
+            t = self._drafts_h
+        self.meta["token_ids"].view(self.B, self.q)[:, 1:].copy_(t, non_blocking=True)
+        self._h2d_done.record()
+
+    def advance(self):
+        r, m = self.r, self.meta
+        rc = lib().mrs_decode_advance_multi(
+            ctypes.c_void_p(r.block_tables.data_ptr()), ctypes.c_int(r.max_blocks), ctypes.c_void_p(r.context_lens.data_ptr()),
+            ctypes.c_int(self.B), ctypes.c_int(r.cfg.block_size), ctypes.c_int(r.split_pages), ctypes.c_int(r.padded_tiles),
+            *[ctypes.c_void_p(m[n].data_ptr()) for n in ("positions", "slot_mapping", "kv_indptr", "kv_indices",
+                                                         "kv_last_page_len", "request_indices", "kv_tile_indices",
+                                                         "o_indptr", "kv_chunk_size", "block_valid_mask")],
+            ctypes.c_int(r.cfg.max_pos), ctypes.c_void_p(r.error_flag.data_ptr()), ctypes.c_int(self.q), r._stream())
+        if rc != 0:
+            raise RuntimeError(f"mrs_decode_advance_multi failed: cudaError {rc}")
+
+    def forward(self):
+        res = self.results
+        rc = lib().mrs_llama_verify_step(ctypes.byref(self.step_struct), ctypes.c_int(self.q),
+                                         ctypes.c_void_p(self.r.context_lens.data_ptr()), ctypes.c_void_p(res.data_ptr()),
+                                         ctypes.c_void_p(res.data_ptr() + 4 * self.B), self.r._stream())
+        if rc != 0:
+            raise RuntimeError(f"mrs_llama_verify_step failed: cudaError {rc}")
+
+    def step(self):
+        """one verify step on the current anchors and drafts (eager): advance by q rows, verify, accept."""
+        self.advance()
+        self.forward()
+
+    def capture(self):
+        """capture step() as a CUDA graph.  The warm-up step outside the capture only writes cache rows past every
+        context; the lengths, the error flag and the anchors are restored."""
+        r = self.r
+        saved = (r.context_lens.clone(), r.error_flag.clone(), self.meta["token_ids"].clone())
+        self.step()
+        r.context_lens.copy_(saved[0]); r.error_flag.copy_(saved[1]); self.meta["token_ids"].copy_(saved[2])
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.step()
+        self.graph = g
+        return g
+
+    def replay(self):
+        self.graph.replay()
+
+    def accepted(self):
+        """[B] device int32: drafts accepted by the last step (-1: the sequence ran out of context and was frozen)"""
+        return self.results[:self.B]
+
+    def emitted(self):
+        """[B, q] device int32: the tokens the last step produced (accepted + 1 per sequence), -1 beyond them"""
+        return self.results[self.B:].view(self.B, self.q)
+
+    def logits(self):
+        """[B*q, vocab]: the target's logits after each fed row"""
+        return self.buf["logits"]
+
+    def fetch(self):
+        """(accepted [B], emitted [B][q]) on the host after one D2H copy"""
+        self._results_h.copy_(self.results, non_blocking=True)
+        torch.cuda.current_stream(self.dev).synchronize()
+        h = self._results_h.tolist()
+        return h[:self.B], [h[self.B + b * self.q:self.B + (b + 1) * self.q] for b in range(self.B)]
+
+
+def speculative_generate(verifier: LlamaVerifier, first_tokens, n_tokens, propose):
+    """Greedy speculative generation: every sequence b starts from first_tokens[b] (processed at position
+    runner.context_lens[b]) and runs until it has produced n_tokens tokens.  propose(history) -> k draft ids, where
+    history is the sequence's tokens so far (first token included).  Per step: one pinned H2D copy of the drafts, one
+    graph replay, one D2H copy of accepted / emitted.  Returns (token streams [B][n_tokens], accepted counts per step
+    [steps][B]); the runner's token_ids hold the next anchors afterwards."""
+    v = verifier
+    if len(first_tokens) != v.B:
+        raise ValueError(f"need {v.B} first tokens, got {len(first_tokens)}")
+    v.r.set_tokens(list(first_tokens))
+    v.sync_from_runner()
+    if v.graph is None:
+        v.capture()
+    hist = [[int(t)] for t in first_tokens]
+    streams = [[] for _ in range(v.B)]
+    steps = []
+    while min(len(s) for s in streams) < n_tokens:
+        v.set_drafts([[int(t) for t in propose(h)] for h in hist])
+        v.replay()
+        acc, em = v.fetch()
+        if min(acc) < 0:
+            raise RuntimeError("speculative_generate: a sequence ran past its allocated context")
+        for b in range(v.B):
+            toks = em[b][:acc[b] + 1]
+            streams[b] += toks
+            hist[b] += toks
+        steps.append(acc)
+    v.sync_to_runner()
+    return [s[:n_tokens] for s in streams], steps
