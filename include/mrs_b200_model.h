@@ -58,7 +58,7 @@ typedef struct {
   const void *final_norm, *rope_cos, *rope_sin; /* rope tables [max_pos, head_dim/2] act dtype */
   /* per-step device metadata (see mrs_decode_advance) */
   int32_t batch, padded_tiles, max_blocks_per_seq;
-  int32_t skip_mask;         /* measurement only: bit0 skip rope/cache/attention, bit1 skip the GEMVs */
+  int32_t skip_mask;         /* measurement only: bit0 skip rope/cache/attention, bit1 skip the GEMVs / GEMMs */
   int32_t fused_attention;   /* 1: mrs_paged_decode_fused; 0: rotary + reshape_and_cache + flashinfer_decode */
   int32_t reserved0;
   int32_t *token_ids;        /* [batch] in: token to process; out_token may alias it */
@@ -77,9 +77,17 @@ typedef struct {
   void (*all_reduce)(void *buf, int64_t count, int32_t dtype, void *stream, void *user);
   void *all_reduce_user;
   const mrs_tp_ctx *tp;      /* non-NULL with world > 1: peer-memory sum (takes precedence over all_reduce) */
+  void *h;                   /* [batch, hidden] normed-activation scratch; read only when batch > 8 */
 } mrs_llama_step;
 
-/* Enqueue one decode step (all layers + lm_head + argmax) on `stream`. Returns cudaError. */
+/* Enqueue one decode step (all layers + lm_head + argmax) on `stream`. Returns cudaError.  batch 1..256.
+ * batch 1..8: the GEMV chain above (Q8_1 activations, MMVQ numerics).
+ * batch 9..256: the reference's MMQ branch — every linear is the wgmma dequant GEMM (mrs_mmq_gguf_grouped: weights
+ * dequantised with the f32 formula and rounded once to the activation format, activations unquantised, f32
+ * accumulation, the prefill GEMM's numerics).  Per layer: grouped QKV (one launch, or q|k + v when attn_v has its own
+ * type) -> the same attention -> o GEMM -> add + RMSNorm -> gate|up GEMM with the SiLU*mul epilogue -> down GEMM
+ * -> add + RMSNorm with the next layer's norm; then the lm_head GEMM and argmax.  Needs `h`; skip_mask bit 1 skips
+ * the GEMMs; cudaErrorInvalidValue with tp or all_reduce set (no tensor parallelism above 8 rows). */
 int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream);
 
 /* On-device restatement of the scheduler-side index producers for a running decode batch

@@ -77,6 +77,17 @@ int mrs_mmvq_fused_qkv_mixed(int type_qk, int type_v, int dt, const void *wq, co
  * launch_mmq_gguf_<q> (REF fast_mmq.rs:102-185): no activation quantisation pass. */
 int32_t mrs_mmq_gguf(int32_t ggml_type, const void *w, const void *x, void *y, int32_t M, int32_t N, int32_t K,
                      int32_t dtype, void *stream);
+/* The ggml-block dequant GEMM (mrs_mmq_gguf's kernel and numerics) over n_mats = 1..3 matrices of one ggml type that
+ * share X [M, K] (q|k|v, gate|up), in one launch: Y_m [M, rows[m]] = X . W_m^T, every W_m [rows[m], K] in its own
+ * buffer, every Y_m row-major in its own buffer (host arrays w, rows, y of n_mats entries).
+ * glu != 0: n_mats == 2, W_0 = gate and W_1 = up with rows[0] == rows[1]; only y[0] is written (y[1] may be NULL),
+ * y[0] = T(silu(T(X . W_0^T))) * T(X . W_1^T) with the product rounded in T, as fused_glu.
+ * pdl != 0: a link of a programmatic-dependent-launch chain — the weights stream before the upstream grid completes,
+ * X is read and Y written after; the launch before it on `stream` must be a link or a plain kernel.
+ * dtype 0 f16, 1 bf16; K % 64 == 0 (% 256 for k-quants); w, x 16-byte aligned, y 2-byte aligned.  0 or a cudaError
+ * (cudaErrorInvalidValue for a bad type, count or shape, cudaErrorMisalignedAddress).  Kernel: csrc/mmq_tc.cu. */
+int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const void **w, const int32_t *rows, void **y,
+                             const void *x, int32_t M, int32_t K, int32_t dtype, int32_t glu, int32_t pdl, void *stream);
 
 /* GPTQ / AWQ int4 linear from the raw checkpoint tensors (no Marlin repack) on the same
  * wgmma kernel: Y[M,N] f16 = X[M,K] f16 . W; GPTQ qweight [K/8,N] (w = (q-8)*s, optional

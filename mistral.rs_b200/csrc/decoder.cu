@@ -19,6 +19,13 @@ extern "C" int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, c
 extern "C" int mrs_mmvq_fused_qkv_mixed(int type_qk, int type_v, int dt, const void *wq, const void *wk, const void *wv,
                                         const void *x, const void *norm_w, float eps, void *q, void *k, void *v,
                                         int K, int nq, int nk, int nv, int b_size, int pdl, void *stream);
+extern "C" int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const void **w, const int32_t *rows,
+                                        void **y, const void *x, int32_t M, int32_t K, int32_t dtype, int32_t glu,
+                                        int32_t pdl, void *stream);
+extern "C" void mrs_rms_norm_f16(const void *x, const void *weight, void *dst, const int nrows, const int ncols, const float eps, int64_t stream);
+extern "C" void mrs_rms_norm_bf16(const void *x, const void *weight, void *dst, const int nrows, const int ncols, const float eps, int64_t stream);
+extern "C" void mrs_add_rms_norm_pdl(const void *x, const void *residual, const void *weight, void *residual_dst, void *norm_dst,
+                                     int32_t nrows, int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream);
 extern "C" void rotary_embedding_positions(void *query, void *key, void *cos_cache, void *sin_cache, void *positions,
                                            int32_t is_neox, int32_t head_size, int64_t num_tokens, int32_t rot_dim,
                                            int32_t seq_len, int32_t num_heads, int32_t num_kv_heads,
@@ -558,9 +565,106 @@ static int32_t llama_forward(const mrs_llama_step *s, int q_len, void *stream) {
   return 0;
 }
 
+// the decode step for 9..256 sequences: the reference's GgmlMatMul sends batches above 8 rows to MMQ, so the linears are
+// the wgmma dequant GEMM (mrs_mmq_gguf_grouped) with the prefill GEMM's numerics.  The norms are their own launches
+// (the GEMM reads X through the TMA, unmodified), into the normed-activation buffer s->h.  Per layer:
+//   grouped QKV -> attention (as the GEMV route) -> o GEMM (into h) -> add + RMSNorm (x2 = o + x, h = norm)
+//   -> gate|up GEMM with the GLU epilogue (act) -> down GEMM (into h) -> add + RMSNorm (x = down + x2, h = next norm)
+// The o and down GEMMs write into h, which the add + RMSNorm after them reads as its input and overwrites with the
+// norm: the norm kernel reads a row's input before its block-wide reduction and writes the row after it.
+// then the lm_head GEMM on h and argmax.  Every launch after the embedding gather and the first norm is a link of the
+// PDL chain when s->pdl is set.
+static int32_t llama_forward_gemm(const mrs_llama_step *s, void *stream) {
+  const int dt = s->act_dtype, B = s->batch, H = s->hidden, pdl = s->pdl;
+  const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool do_attn = !(s->skip_mask & 1), do_gemm = !(s->skip_mask & 2);
+  if (s->h == nullptr || (dt != MRS_F16 && dt != MRS_BF16)) return (int32_t)cudaErrorInvalidValue;
+  auto gemm = [&](int type, int n, const void **w, const int32_t *rows, void **y, const void *x, int K, int glu) {
+    return mrs_mmq_gguf_grouped(type, n, w, rows, y, x, B, K, dt, glu, pdl, stream);
+  };
+  auto add_rms = [&](const void *x, const void *res, const void *w, void *res_dst) {
+    mrs_add_rms_norm_pdl(x, res, w, res_dst, s->h, B, H, s->rms_eps, dt, pdl, stream);
+  };
+
+  MRS_TRY(mrs_embedding_gather(s->tok_embd.ggml_type, s->tok_embd.data, H, s->token_ids, B, s->x, dt, stream));
+  if (dt == MRS_F16) mrs_rms_norm_f16(s->x, s->layers[0].attn_norm, s->h, B, H, s->rms_eps, (int64_t)stream);
+  else mrs_rms_norm_bf16(s->x, s->layers[0].attn_norm, s->h, B, H, s->rms_eps, (int64_t)stream);
+  for (int l = 0; l < s->n_layers; l++) {
+    const mrs_llama_layer &L = s->layers[l];
+    if (do_gemm) {
+      const void *w[3] = {L.wq.data, L.wk.data, L.wv.data};
+      int32_t rows[3] = {nq, nkv, nkv};
+      void *y[3] = {s->q, s->k, s->v};
+      if (L.wq.ggml_type == L.wk.ggml_type && L.wk.ggml_type == L.wv.ggml_type) {
+        MRS_TRY(gemm(L.wq.ggml_type, 3, w, rows, y, s->h, H, 0));
+      } else if (L.wq.ggml_type == L.wk.ggml_type) {   // Q4_K_M keeps attn_v in Q6_K on some layers
+        MRS_TRY(gemm(L.wq.ggml_type, 2, w, rows, y, s->h, H, 0));
+        MRS_TRY(gemm(L.wv.ggml_type, 1, w + 2, rows + 2, y + 2, s->h, H, 0));
+      } else {
+        const int types[3] = {L.wq.ggml_type, L.wk.ggml_type, L.wv.ggml_type};
+        for (int m = 0; m < 3; m++) MRS_TRY(gemm(types[m], 1, w + m, rows + m, y + m, s->h, H, 0));
+      }
+    }
+    if (do_attn && s->fused_attention) {
+      MRS_TRY(mrs_paged_decode_fused(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
+                                     s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
+                                     s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
+                                     s->block_valid_mask, s->attn_out, s->padded_tiles > B ? s->tmp_v : nullptr,
+                                     s->padded_tiles > B ? s->tmp_s : nullptr, s->attn_counters, B, s->padded_tiles,
+                                     s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
+                                     pdl | (s->rope_neox ? 0 : 2), stream));
+    } else if (do_attn) {
+      rotary_embedding_positions(s->q, s->k, (void *)s->rope_cos, (void *)s->rope_sin, s->positions, s->rope_neox,
+                                 s->head_dim, B, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt,
+                                 (int64_t)stream);
+      reshape_and_cache_flashinfer(s->k, s->v, L.k_cache, L.v_cache, s->slot_mapping, B, s->n_kv_heads, s->head_dim,
+                                   s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
+      MRS_TRY(flashinfer_decode(s->q, L.k_cache, L.v_cache, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
+                                s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
+                                (const bool *)s->block_valid_mask, s->attn_out, s->padded_tiles > B ? s->tmp_v : nullptr,
+                                s->padded_tiles > B ? s->tmp_s : nullptr, B, s->padded_tiles, s->n_heads, s->n_kv_heads,
+                                s->head_dim, s->block_size, nq, s->head_dim, s->sm_scale, -1, 0.f, 1.f, 1.f,
+                                (uint32_t)dt, (uint32_t)dt, st));
+    }
+    if (!do_gemm) continue;
+    {
+      const void *w[1] = {L.wo.data};
+      const int32_t rows[1] = {H};
+      void *y[1] = {s->h};
+      MRS_TRY(gemm(L.wo.ggml_type, 1, w, rows, y, s->attn_out, nq, 0));
+    }
+    add_rms(s->h, s->x, L.ffn_norm, s->x2);                                     // x2 = o + x ; h = norm(x2)
+    if (L.w_gate.ggml_type != L.w_up.ggml_type || L.w_gate.rows != L.w_up.rows) return (int32_t)cudaErrorInvalidValue;
+    {
+      const void *w[2] = {L.w_gate.data, L.w_up.data};
+      const int32_t rows[2] = {L.w_gate.rows, L.w_up.rows};
+      void *y[2] = {s->act, nullptr};
+      MRS_TRY(gemm(L.w_gate.ggml_type, 2, w, rows, y, s->h, H, 1));
+    }
+    {
+      const void *w[1] = {L.w_down.data};
+      const int32_t rows[1] = {H};
+      void *y[1] = {s->h};
+      MRS_TRY(gemm(L.w_down.ggml_type, 1, w, rows, y, s->act, L.w_down.cols, 0));
+    }
+    add_rms(s->h, s->x2, l + 1 < s->n_layers ? s->layers[l + 1].attn_norm : s->final_norm, s->x);   // x = down + x2 ; h = next norm(x)
+  }
+  if (do_gemm) {
+    const void *w[1] = {s->lm_head.data};
+    const int32_t rows[1] = {s->vocab};
+    void *y[1] = {s->logits};
+    MRS_TRY(gemm(s->lm_head.ggml_type, 1, w, rows, y, s->h, H, 0));
+  }
+  MRS_TRY(mrs_argmax(s->logits, B, s->vocab, dt, s->out_token, s->argmax_scratch, pdl, stream));
+  return (int32_t)cudaGetLastError();
+}
+
 extern "C" int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream) {
-  if (s->batch < 1 || s->batch > 8) return (int32_t)cudaErrorInvalidValue;
-  return llama_forward(s, 1, stream);
+  if (s->batch < 1 || s->batch > 256) return (int32_t)cudaErrorInvalidValue;
+  if (s->batch <= 8) return llama_forward(s, 1, stream);
+  if (s->tp != nullptr || s->all_reduce != nullptr) return (int32_t)cudaErrorInvalidValue;
+  return llama_forward_gemm(s, stream);
 }
 
 extern "C" int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,

@@ -182,6 +182,44 @@ template <int TYPE> struct GgmlSrc {
     for (int i = 0; i < 16; i++) o[i] = pack_act2(v[2 * i], v[2 * i + 1], bf != 0);
   }
 };
+// up to three ggml matrices of one type over the same X and K (q|k|v, gate|up), each in its own buffer with its own
+// output [M, rows_m].  Grouped (GLU false): global weight row n runs through matrix 0, then 1, then 2; a 128-row tile
+// may straddle two matrices, so every row is mapped on its own.  GLU: tile z holds gate rows 64 z .. 64 z + 63 in its
+// first 64 rows and the same up rows in its second 64 (warpgroup 0 / 1); only the gate rows' outputs are written.
+template <int TYPE, bool GLU> struct GgmlGroupSrc {
+  static constexpr bool kTmaA = false;
+  static constexpr int kAhead = 1;
+  static constexpr int kEpi = GLU ? 2 : 1;
+  using Raw = Raw32<TYPE>;
+  const uint8_t *w0, *w1, *w2;
+  void *y0, *y1, *y2;
+  int r0, r1, r2;          // rows (output widths) of the matrices; 0 for an absent one
+  int row_bytes, bf;
+  __device__ __forceinline__ int mat(int n) const { return GLU ? (n >> 6) & 1 : (n >= r0) + (n >= r0 + r1); }
+  __device__ __forceinline__ int local(int n, int m) const {
+    return GLU ? (n >> 7) * 64 + (n & 63) : n - (m == 0 ? 0 : m == 1 ? r0 : r0 + r1);
+  }
+  __device__ __forceinline__ bool live(int n) const {
+    const int m = mat(n);
+    return local(n, m) < (m == 0 ? r0 : m == 1 ? r1 : r2);
+  }
+  __device__ __forceinline__ const uint8_t *wrow(int n) const {
+    const int m = mat(n);
+    return (m == 0 ? w0 : m == 1 ? w1 : w2) + (size_t)local(n, m) * row_bytes;
+  }
+  __device__ __forceinline__ void *out(int n, int tok) const {
+    const int m = mat(n);
+    const int width = m == 0 ? r0 : m == 1 ? r1 : r2;
+    return (uint16_t *)(m == 0 ? y0 : m == 1 ? y1 : y2) + (size_t)tok * width + local(n, m);
+  }
+  __device__ __forceinline__ void load(Raw &r, int row, int k) const { load_raw32<TYPE>(wrow(row), k, r); }
+  __device__ __forceinline__ void expand(const Raw &r, int row, int k, uint32_t *o) const {
+    float v[32];
+    expand32<TYPE>(r, wrow(row), k, v);
+#pragma unroll
+    for (int i = 0; i < 16; i++) o[i] = pack_act2(v[2 * i], v[2 * i + 1], bf != 0);
+  }
+};
 // GPTQ / AWQ checkpoints and packed-affine weights: separate arrays read through dequant32_ckpt
 template <int TYPE> struct CkptSrc {
   static constexpr bool kTmaA = false;
@@ -235,6 +273,62 @@ extern "C" int32_t mrs_mmq_gguf(int32_t ggml_type, const void *w, const void *x,
   default: return (int32_t)cudaErrorInvalidValue;
   }
 #undef MRS_G
+}
+
+template <bool GLU>
+static cudaError_t mmq_group_run(int type, const GgmlGroupSrc<MRS_Q4_0, GLU> &a, const void *x, int M, int N, int K, int dtype,
+                                 int pdl, cudaStream_t st) {
+  // one field layout for every type: only the decoder differs
+#define MRS_GG(T) return hg_run(GgmlGroupSrc<T, GLU>{a.w0, a.w1, a.w2, a.y0, a.y1, a.y2, a.r0, a.r1, a.r2, a.row_bytes, a.bf}, \
+                                x, nullptr, nullptr, M, N, K, dtype, pdl, st)
+  switch (type) {
+  case MRS_Q4_0: MRS_GG(MRS_Q4_0);
+  case MRS_Q4_1: MRS_GG(MRS_Q4_1);
+  case MRS_Q5_0: MRS_GG(MRS_Q5_0);
+  case MRS_Q5_1: MRS_GG(MRS_Q5_1);
+  case MRS_Q8_0: MRS_GG(MRS_Q8_0);
+  case MRS_Q2_K: MRS_GG(MRS_Q2_K);
+  case MRS_Q3_K: MRS_GG(MRS_Q3_K);
+  case MRS_Q4_K: MRS_GG(MRS_Q4_K);
+  case MRS_Q5_K: MRS_GG(MRS_Q5_K);
+  case MRS_Q6_K: MRS_GG(MRS_Q6_K);
+  default: return cudaErrorInvalidValue;
+  }
+#undef MRS_GG
+}
+
+// The GEMM over n_mats (1..3) ggml matrices of one type that share X [M, K]: Y_m [M, rows[m]] = X . W_m^T, one launch
+// (q|k|v, gate|up, or a single matrix as a link of a PDL chain).  glu != 0: n_mats == 2, W_0 = gate and W_1 = up of
+// equal rows, and only y[0] = T(silu(T(X . W_0^T))) * T(X . W_1^T) (in T, as fused_glu) is written.  pdl != 0: a link
+// of a programmatic-dependent-launch chain (weights stream before the upstream grid completes; x is read and y written
+// after).  Same numerics and checks as mrs_mmq_gguf.
+extern "C" int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const void **w, const int32_t *rows,
+                                        void **y, const void *x, int32_t M, int32_t K, int32_t dtype, int32_t glu,
+                                        int32_t pdl, void *stream) {
+  if (n_mats < 1 || n_mats > 3 || w == nullptr || rows == nullptr || y == nullptr) return (int32_t)cudaErrorInvalidValue;
+  if (glu && (n_mats != 2 || rows[0] != rows[1])) return (int32_t)cudaErrorInvalidValue;
+  if (M <= 0) return 0;
+  const int rb = tc_row_bytes(ggml_type, K);
+  if (rb == 0 || K % 64 != 0 || (dtype != 0 && dtype != 1)) return (int32_t)cudaErrorInvalidValue;
+  if (ggml_type >= MRS_Q2_K && K % 256 != 0) return (int32_t)cudaErrorInvalidValue;
+  if ((uintptr_t)x & 15) return (int32_t)cudaErrorMisalignedAddress;
+  int64_t total = 0;
+  for (int m = 0; m < n_mats; m++) {
+    if (rows[m] <= 0 || w[m] == nullptr || (y[m] == nullptr && !(glu && m == 1))) return (int32_t)cudaErrorInvalidValue;
+    if (((uintptr_t)w[m] & 15) || ((uintptr_t)y[m] & 1)) return (int32_t)cudaErrorMisalignedAddress;
+    total += rows[m];
+  }
+  if (total > (int64_t)1 << 30) return (int32_t)cudaErrorInvalidValue;
+  const int n = n_mats;
+  GgmlGroupSrc<MRS_Q4_0, false> a{(const uint8_t *)w[0], n > 1 ? (const uint8_t *)w[1] : nullptr, n > 2 ? (const uint8_t *)w[2] : nullptr,
+                                  y[0], n > 1 ? y[1] : nullptr, n > 2 ? y[2] : nullptr, rows[0], n > 1 ? rows[1] : 0,
+                                  n > 2 ? rows[2] : 0, rb, dtype};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (glu) {
+    const GgmlGroupSrc<MRS_Q4_0, true> g{a.w0, a.w1, nullptr, a.y0, a.y1, nullptr, a.r0, a.r1, 0, rb, dtype};
+    return (int32_t)mmq_group_run<true>(ggml_type, g, x, M, (rows[0] + 63) / 64 * HG_BM, K, dtype, pdl, st);
+  }
+  return (int32_t)mmq_group_run<false>(ggml_type, a, x, M, (int)total, K, dtype, pdl, st);
 }
 
 // GPTQ / AWQ int4 linear on the tensor cores, straight from the checkpoint tensors (no Marlin

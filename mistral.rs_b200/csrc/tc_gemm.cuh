@@ -74,6 +74,17 @@ __device__ __forceinline__ uint32_t pack_act2(float lo, float hi, bool bf) {
   return *(const uint32_t *)&h;
 }
 
+// Epilogue of a source: 0 (default) writes y[M, N]; a source with `static constexpr int kEpi` 1 owns its row map:
+// `live(row)` says whether weight row `row` exists and `out(row, tok)` is where its output goes (several matrices
+// with their own outputs in one launch); kEpi 2 (GLU) additionally pairs the two warpgroups: warpgroup 1's rows are
+// the up rows of warpgroup 0's gate rows, and only warpgroup 0 writes, act(T(gate)) * T(up) in T.
+template <class S> __host__ __device__ constexpr auto hg_epi_kind(int) -> decltype(S::kEpi, int()) { return S::kEpi; }
+template <class S> __host__ __device__ constexpr int hg_epi_kind(long) { return 0; }
+template <class Src> __device__ __forceinline__ bool hg_row_live(const Src &src, int row, int N) {
+  if constexpr (hg_epi_kind<Src>(0) != 0) return src.live(row);
+  else return row < N;
+}
+
 // Src: struct with `static constexpr bool kTmaA` (A tiles come from the TMA map `tmap_w`, no dequantisation),
 // `static constexpr int kAhead` (how many 64-k steps of raw weights a thread keeps in flight in registers), a
 // per-thread `Raw` state, `load(Raw &, row, k)` (issues the loads of weights k .. k+31 of `row`) and
@@ -136,7 +147,7 @@ hg_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CU
   const int g = warp >> 2, t = tid & 127;
   const int r = 64 * g + (t >> 1), hf = t & 1;   // weight row in the tile, which 32-k half of the step
   const int row = n0 + r;
-  const bool live = row < p.N;
+  const bool live = hg_row_live(src, row, p.N);
   float acc[NACC];
 #pragma unroll
   for (int i = 0; i < NACC; i++) acc[i] = 0.f;
@@ -216,18 +227,55 @@ hg_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CU
         for (int e = 0; e < 4; e++) acc[4 * j + e] += rp[(8 * j + tc + (e & 1)) * HG_BM + wr + 8 * (e >> 1)];
     }
   }
-  // PDL: y may only be overwritten once the upstream grid has completed
-  if (p.pdl) pdl_wait();
+  constexpr int EPI = hg_epi_kind<Src>(0);
+  if constexpr (EPI == 2) {
+    // GLU: thread t of warpgroup 1 holds, register for register, the up values of thread t of warpgroup 0's gate
+    // values.  They pass rounded to T through the A ring, free once both warpgroups' MMAs have retired.
+    uint16_t *xch = (uint16_t *)a_ring;   // [NACC][128]
+    asm volatile("bar.sync 3, 256;" ::: "memory");
+    if (g == 1) {
 #pragma unroll
-  for (int j = 0; j < NT / 8; j++)
-#pragma unroll
-    for (int e = 0; e < 4; e++) {
-      const int tok = m0 + 8 * j + tc + (e & 1), n = n0 + wr + 8 * (e >> 1);
-      if (tok < p.M && n < p.N) {
-        if constexpr (BF) ((__nv_bfloat16 *)p.y)[(size_t)tok * p.N + n] = __float2bfloat16_rn(acc[4 * j + e]);
-        else ((__half *)p.y)[(size_t)tok * p.N + n] = __float2half_rn(acc[4 * j + e]);
+      for (int i = 0; i < NACC; i++) {
+        if constexpr (BF) xch[i * 128 + t] = __bfloat16_as_ushort(__float2bfloat16_rn(acc[i]));
+        else xch[i * 128 + t] = __half_as_ushort(__float2half_rn(acc[i]));
       }
     }
+    asm volatile("bar.sync 3, 256;" ::: "memory");
+    if (g == 1) return;
+  }
+  // PDL: y may only be overwritten once the upstream grid has completed
+  if (p.pdl) pdl_wait();
+  if constexpr (EPI == 0) {
+#pragma unroll
+    for (int j = 0; j < NT / 8; j++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) {
+        const int tok = m0 + 8 * j + tc + (e & 1), n = n0 + wr + 8 * (e >> 1);
+        if (tok < p.M && n < p.N) {
+          if constexpr (BF) ((__nv_bfloat16 *)p.y)[(size_t)tok * p.N + n] = __float2bfloat16_rn(acc[4 * j + e]);
+          else ((__half *)p.y)[(size_t)tok * p.N + n] = __float2half_rn(acc[4 * j + e]);
+        }
+      }
+  } else {
+#pragma unroll
+    for (int j = 0; j < NT / 8; j++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) {
+        const int tok = m0 + 8 * j + tc + (e & 1), n = n0 + wr + 8 * (e >> 1);
+        if (tok < p.M && src.live(n)) {
+          float v = acc[4 * j + e];
+          if constexpr (EPI == 2) {   // as fused_glu: T(act(f32(T(gate)))), then the product in T
+            const uint16_t u = ((const uint16_t *)a_ring)[(4 * j + e) * 128 + t];
+            const float up = BF ? __bfloat162float(__ushort_as_bfloat16(u)) : __half2float(__ushort_as_half(u));
+            const float gt = BF ? __bfloat162float(__float2bfloat16_rn(v)) : __half2float(__float2half_rn(v));
+            const float a = glu_activation(gt, 0);
+            v = (BF ? __bfloat162float(__float2bfloat16_rn(a)) : __half2float(__float2half_rn(a))) * up;
+          }
+          if constexpr (BF) *(__nv_bfloat16 *)src.out(n, tok) = __float2bfloat16_rn(v);
+          else *(__half *)src.out(n, tok) = __float2half_rn(v);
+        }
+      }
+  }
 }
 
 // split K over a cluster when the row tiles alone leave SMs idle.  Splits are whole 64-k steps; the partials take

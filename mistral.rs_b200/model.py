@@ -131,7 +131,7 @@ class _Step(ctypes.Structure):
                                                "kv_chunk_size", "block_valid_mask", "x", "x2", "q", "k", "v",
                                                "attn_out", "act", "logits", "tmp_v", "tmp_s", "out_token",
                                                "attn_counters", "argmax_scratch")] + \
-               [("all_reduce", _AR_FN), ("all_reduce_user", ctypes.c_void_p), ("tp", ctypes.c_void_p)]
+               [("all_reduce", _AR_FN), ("all_reduce_user", ctypes.c_void_p), ("tp", ctypes.c_void_p), ("h", ctypes.c_void_p)]
 
 
 class _TpCtx(ctypes.Structure):
@@ -510,12 +510,28 @@ def runner_split_pages(block_size, batch, n_kv_heads, max_ctx, sm_count=132, min
     return max(1, -(-tokens // block_size))
 
 
+MAX_DECODE_BATCH = 256   # sequences per decode step (mrs_decode_advance / mrs_llama_decode_step)
+MMVQ_MAX_BATCH = 8       # up to this many rows the linears are GEMVs; above, the dequant GEMM (the reference's MMQ branch)
+
+
+def check_runner_args(batch, comm=None, peer_allreduce=None):
+    """ValueError for a decode batch mrs_llama_decode_step rejects: outside 1..256, or tensor parallel above 8 rows."""
+    if isinstance(batch, bool) or not isinstance(batch, (int, np.integer)) or not 1 <= batch <= MAX_DECODE_BATCH:
+        raise ValueError(f"LlamaRunner: batch must be an int in 1..{MAX_DECODE_BATCH}, got {batch!r}")
+    if batch > MMVQ_MAX_BATCH and (comm is not None or peer_allreduce is not None):
+        raise ValueError(f"LlamaRunner: tensor parallelism (comm / peer_allreduce) runs batches of up to {MMVQ_MAX_BATCH}, "
+                         f"got {batch}")
+
+
 class LlamaRunner:
     """Owns KV cache + scratch + per-step metadata for a batch of sequences and drives
-    mrs_llama_decode_step / mrs_decode_advance (eagerly or as a captured CUDA graph)."""
+    mrs_llama_decode_step / mrs_decode_advance (eagerly or as a captured CUDA graph).
+    batch 1..8 runs the GEMV chain, 9..256 the dequant-GEMM chain (prefill numerics; see mrs_b200_model.h)."""
 
     def __init__(self, weights: LlamaWeights, batch=1, max_ctx=512, pdl=False, sm_count=132, comm=None,
                  fused_attention=True, split_policy="sm_fill", split_min_tokens=64, peer_allreduce=None):
+        check_runner_args(batch, comm, peer_allreduce)
+        batch = int(batch)
         cfg, dev, dt = weights.cfg, weights.device, weights.dtype
         self.w, self.cfg, self.dev, self.dt, self.B = weights, cfg, dev, dt, batch
         tp = weights.tp_size
@@ -550,7 +566,8 @@ class LlamaRunner:
                         tmp_s=torch.zeros(self.padded_tiles, self.n_heads, dtype=torch.float32, device=dev),
                         out_token=self.meta["token_ids"],  # argmax feeds the next step directly
                         attn_counters=torch.zeros(batch * self.n_kv * 2, dtype=torch.int32, device=dev),
-                        argmax_scratch=torch.zeros(16 * batch + 16, dtype=torch.uint8, device=dev))
+                        argmax_scratch=torch.zeros(16 * batch + 16, dtype=torch.uint8, device=dev),
+                        h=a(batch, H))
         self.k_cache = [a(nb, self.n_kv, bs, cfg.head_dim) for _ in range(cfg.n_layers)]
         self.v_cache = [a(nb, self.n_kv, bs, cfg.head_dim) for _ in range(cfg.n_layers)]
         self._layers = (_Layer * cfg.n_layers)()
@@ -618,9 +635,20 @@ class LlamaRunner:
         self.forward()
 
     def reset(self, context_len=0):
-        self.context_lens.fill_(context_len)
+        """context_len: one length for every sequence, or a sequence of B lengths (sequences at different positions,
+        e.g. prompts of different lengths prefilled into their own tables).  The host-side bound on further steps
+        follows the longest."""
+        if isinstance(context_len, (int, np.integer)):
+            self.context_lens.fill_(int(context_len))
+            longest = int(context_len)
+        else:
+            lens = [int(c) for c in context_len]
+            if len(lens) != self.B or min(lens) < 0:
+                raise ValueError(f"LlamaRunner.reset: need {self.B} lengths >= 0, got {lens}")
+            self.context_lens.copy_(torch.tensor(lens, dtype=torch.int32))
+            longest = max(lens)
         self.error_flag.zero_()
-        self.steps_taken = int(context_len)
+        self.steps_taken = longest
 
     def replay(self):
         """one captured decode step; raises before a sequence would run past the allocated context
