@@ -77,7 +77,8 @@ typedef struct {
   void (*all_reduce)(void *buf, int64_t count, int32_t dtype, void *stream, void *user);
   void *all_reduce_user;
   const mrs_tp_ctx *tp;      /* non-NULL with world > 1: peer-memory sum (takes precedence over all_reduce) */
-  void *h;                   /* [batch, hidden] normed-activation scratch; read only when batch > 8 */
+  void *h;                   /* [batch, hidden] normed-activation scratch ([batch*q_len, hidden] for a verify step);
+                              * read only when batch > 8 */
 } mrs_llama_step;
 
 /* Enqueue one decode step (all layers + lm_head + argmax) on `stream`. Returns cudaError.  batch 1..256.
@@ -119,13 +120,19 @@ int32_t mrs_decode_advance(const int32_t *block_tables, int32_t max_blocks_per_s
  * emitted all -1 and keeps its context and anchor.
  *
  * mrs_llama_verify_step: s->batch = B sequences, every row buffer of `s` (token_ids, positions, slot_mapping, x, x2,
- * q, k, v, attn_out, act, logits, out_token) holds B*q_len rows, tmp_v / tmp_s hold [padded_tiles, q_len*n_heads],
- * attn_counters B*n_kv_heads*ceil(group*q_len/16), argmax_scratch >= 16*B*q_len + 16 bytes; the metadata comes from
- * mrs_decode_advance_multi.  Embedding gather of the B*q_len ids -> the decode layer chain with the multi-query fused
- * attention -> lm_head on every row -> mrs_argmax into out_token (must not alias token_ids) -> mrs_spec_accept with
- * `context_lens` (the lengths the advance read; the step struct carries none).  Graph-capturable.  skip_mask as for
- * decode.  cudaErrorInvalidValue for B*q_len > 8, q_len outside 2..8, fused_attention == 0, head_dim other than 64 /
- * 128, or tp / all_reduce set. */
+ * q, k, v, attn_out, act, logits, out_token, and h on the GEMM route) holds B*q_len rows, tmp_v / tmp_s hold
+ * [padded_tiles, q_len*n_heads], attn_counters B*n_kv_heads*ceil(group*q_len/16), argmax_scratch >= 16*B*q_len + 16
+ * bytes; the metadata comes from mrs_decode_advance_multi.  Embedding gather of the B*q_len ids -> the decode layer
+ * chain with the multi-query fused attention -> lm_head on every row -> mrs_argmax into out_token (must not alias
+ * token_ids) -> mrs_spec_accept with `context_lens` (the lengths the advance read; the step struct carries none), all
+ * one PDL chain when s->pdl is set.  The linears take the route of mrs_llama_decode_step for the same B, so plain and
+ * verify steps of one batch share their numerics:
+ *   B 1..8:   the GEMV chain, B*q_len <= 8 rows;
+ *   B 9..256: the wgmma dequant-GEMM chain (prefill GEMM numerics) over B*q_len rows, up to 2048; needs `h` and an
+ *             f16 / bf16 activation dtype.
+ * Graph-capturable.  skip_mask as for decode.  cudaErrorInvalidValue for B outside 1..256, B <= 8 with B*q_len > 8,
+ * q_len outside 2..8, fused_attention == 0, head_dim other than 64 / 128, tp / all_reduce set, out_token ==
+ * token_ids, a NULL context_lens / accepted / emitted, or (B >= 9) a NULL h or another activation dtype. */
 int32_t mrs_decode_advance_multi(const int32_t *block_tables, int32_t max_blocks_per_seq, int32_t *context_lens,
                                  int32_t batch, int32_t block_size, int32_t split_pages, int32_t padded_tiles,
                                  int32_t *positions, int64_t *slot_mapping, int32_t *kv_indptr, int32_t *kv_indices,

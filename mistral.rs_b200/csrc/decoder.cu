@@ -574,8 +574,11 @@ static int32_t llama_forward(const mrs_llama_step *s, int q_len, void *stream) {
 // norm: the norm kernel reads a row's input before its block-wide reduction and writes the row after it.
 // then the lm_head GEMM on h and argmax.  Every launch after the embedding gather and the first norm is a link of the
 // PDL chain when s->pdl is set.
-static int32_t llama_forward_gemm(const mrs_llama_step *s, void *stream) {
-  const int dt = s->act_dtype, B = s->batch, H = s->hidden, pdl = s->pdl;
+// q_len > 1 is a speculative verify step of the 9..256-sequence route: every row-wise launch covers batch * q_len rows
+// and the attention is mrs_paged_decode_fused_multi over the batch's sequences, as in llama_forward.  q_len == 1
+// issues exactly the decode step's launches.
+static int32_t llama_forward_gemm(const mrs_llama_step *s, int q_len, void *stream) {
+  const int dt = s->act_dtype, NS = s->batch, B = s->batch * q_len, H = s->hidden, pdl = s->pdl;
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
   cudaStream_t st = (cudaStream_t)stream;
   const bool do_attn = !(s->skip_mask & 1), do_gemm = !(s->skip_mask & 2);
@@ -606,7 +609,15 @@ static int32_t llama_forward_gemm(const mrs_llama_step *s, void *stream) {
         for (int m = 0; m < 3; m++) MRS_TRY(gemm(types[m], 1, w + m, rows + m, y + m, s->h, H, 0));
       }
     }
-    if (do_attn && s->fused_attention) {
+    if (do_attn && q_len > 1) {
+      MRS_TRY(mrs_paged_decode_fused_multi(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
+                                           s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
+                                           s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
+                                           s->block_valid_mask, s->attn_out, s->padded_tiles > NS ? s->tmp_v : nullptr,
+                                           s->padded_tiles > NS ? s->tmp_s : nullptr, s->attn_counters, NS, s->padded_tiles,
+                                           s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
+                                           pdl | (s->rope_neox ? 0 : 2), q_len, stream));
+    } else if (do_attn && s->fused_attention) {
       MRS_TRY(mrs_paged_decode_fused(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
                                      s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
                                      s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
@@ -664,16 +675,19 @@ extern "C" int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream) 
   if (s->batch < 1 || s->batch > 256) return (int32_t)cudaErrorInvalidValue;
   if (s->batch <= 8) return llama_forward(s, 1, stream);
   if (s->tp != nullptr || s->all_reduce != nullptr) return (int32_t)cudaErrorInvalidValue;
-  return llama_forward_gemm(s, stream);
+  return llama_forward_gemm(s, 1, stream);
 }
 
+// the verify step takes the linear route of the runner's plain step, chosen by the sequence count: batch 1..8 the GEMV
+// chain (batch * q_len <= 8 rows), batch 9..256 the GEMM chain (up to 2048 rows)
 extern "C" int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,
                                          int32_t *emitted, void *stream) {
-  if (q_len < 2 || q_len > 8 || s->batch < 1 || s->batch * q_len > 8 || s->tp != nullptr || s->all_reduce != nullptr ||
-      !s->fused_attention || (s->head_dim != 64 && s->head_dim != 128) || s->out_token == s->token_ids ||
-      context_lens == nullptr || accepted == nullptr || emitted == nullptr)
+  const bool gemm = s->batch > 8;
+  if (q_len < 2 || q_len > 8 || s->batch < 1 || s->batch > 256 || (!gemm && s->batch * q_len > 8) || s->tp != nullptr ||
+      s->all_reduce != nullptr || !s->fused_attention || (s->head_dim != 64 && s->head_dim != 128) ||
+      s->out_token == s->token_ids || context_lens == nullptr || accepted == nullptr || emitted == nullptr)
     return (int32_t)cudaErrorInvalidValue;
-  MRS_TRY(llama_forward(s, q_len, stream));
+  MRS_TRY(gemm ? llama_forward_gemm(s, q_len, stream) : llama_forward(s, q_len, stream));
   return mrs_spec_accept(s->out_token, s->token_ids, s->slot_mapping, context_lens, accepted, emitted, s->batch, q_len,
                          s->pdl, stream);
 }

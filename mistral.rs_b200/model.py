@@ -797,11 +797,13 @@ def check_drafts(drafts, batch, draft_len, vocab):
 
 
 def check_verifier_args(runner, draft_len):
-    """ValueError unless `runner` can run verify steps of `draft_len` drafts (see LlamaVerifier)."""
+    """ValueError unless `runner` can run verify steps of `draft_len` drafts (see LlamaVerifier).  A verify step takes
+    the linear route of the runner's plain step: up to 8 sequences the GEMV chain, which holds B * (k + 1) <= 8 rows;
+    9..256 sequences the GEMM chain, which takes any k."""
     k = int(draft_len)
     if not 1 <= k <= 7:
         raise ValueError(f"draft_len must be 1..7, got {draft_len}")
-    if runner.B * (k + 1) > 8:
+    if runner.B <= MMVQ_MAX_BATCH and runner.B * (k + 1) > MMVQ_MAX_BATCH:
         raise ValueError(f"batch x (draft_len + 1) = {runner.B} x {k + 1} exceeds the 8 rows of one verify step")
     if runner.w.tp_size != 1 or runner._peer is not None or runner._ar_cb is not None:
         raise ValueError("speculative verification runs single-GPU (no tensor parallelism)")
@@ -820,7 +822,8 @@ class LlamaVerifier:
     """Greedy speculative decoding on a LlamaRunner's sequences (REF mistralrs-core/src/speculative/): each verify step
     feeds q = k + 1 rows per sequence — the anchor (the token the runner would process next) and k caller-proposed
     drafts — through mrs_llama_verify_step in one pass over the weights, and accepts drafts on the device
-    (mrs_spec_accept).
+    (mrs_spec_accept).  Verify steps take the runner's linear route: the GEMV chain for 1..8 sequences (B * q <= 8),
+    the dequant-GEMM chain for 9..256 (B * q up to 2048 rows), so plain and verify steps share their numerics.
 
     Shares the runner's weights, KV caches, block tables, context_lens and error_flag, so verify steps and plain
     `runner.step()` calls can be mixed; owns the B*q-row metadata and scratch.  The anchor moves explicitly:
@@ -846,7 +849,8 @@ class LlamaVerifier:
                         tmp_v=a(r.padded_tiles, q * n_heads, D),
                         tmp_s=torch.zeros(r.padded_tiles, q * n_heads, dtype=torch.float32, device=dev),
                         out_token=z(R), attn_counters=z(B * n_kv * nsub),
-                        argmax_scratch=torch.zeros(16 * R + 16, dtype=torch.uint8, device=dev))
+                        argmax_scratch=torch.zeros(16 * R + 16, dtype=torch.uint8, device=dev),
+                        h=a(R, H))                    # the GEMM route's normed activations (not the runner's [B, H])
         self.results = z(B + R)                       # accepted [B] then emitted [B*q]: one D2H copy per step
         self._results_h = torch.zeros(B + R, dtype=torch.int32).pin_memory()
         self._drafts_h = torch.zeros(B, k, dtype=torch.int32).pin_memory()

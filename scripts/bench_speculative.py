@@ -14,8 +14,14 @@ Prints one JSON line:
                             position corrupted with a seeded probability chosen for a mean acceptance of `target`:
                             tok/s (host clock around work that ends in a device synchronise), mean accepted drafts per
                             step, measured acceptance, and whether the stream equals the plain greedy one
-Usage: python scripts/bench_speculative.py [--replays 200] [--layers N] [--out FILE]"""
+--batch B > 1 runs B sequences, each with its own 128-token prompt prefilled into its own block table.  Batches of 9
+and more take the dequant-GEMM route for plain and verify steps alike, so the step splits are named linear_ms there.
+Step costs are measured at q = 2, 4, 8 (those that fit the 8 rows of the GEMV route when B <= 8); the plain and
+generation rates count the tokens of all B sequences, and generation reports how many of the B streams equal their
+plain greedy stream (with the first differing position of each that does not).
+Usage: python scripts/bench_speculative.py [--batch 1] [--replays 200] [--layers N] [--out FILE]"""
 import argparse
+import itertools
 import json
 import os
 import subprocess
@@ -73,12 +79,43 @@ def corruption_for(target, k):
     return (lo + hi) / 2
 
 
+def step_costs(runner, vers, linear, replays):
+    """step cost: plain decode and verify at q = k + 1 for every verifier, whole and split (`linear`: the name of the
+    linear-only split)"""
+    ctx = PROMPT_LEN + GEN_LEN // 2
+    steps = {}
+    for q in (1,) + tuple(k + 1 for k in vers):
+        s = runner.step_struct if q == 1 else vers[q - 1].step_struct
+        fwd = runner.forward if q == 1 else vers[q - 1].forward
+        row = {}
+        for name, mask in (("total_ms", 0), (linear, 1), ("attention_ms", 2)):
+            s.skip_mask = mask
+            runner.context_lens.fill_(ctx)
+            (runner.advance if q == 1 else vers[q - 1].advance)()      # metadata of a context-`ctx` step
+            row[name] = median_replay_ms(capture_forward(fwd), runner, ctx + q, replays)
+        s.skip_mask = 0
+        row["ms_per_row"] = row["total_ms"] / q
+        steps[q] = row
+    return steps
+
+
+def emit(res, out):
+    line = json.dumps(res)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=1, help="sequences per step (1..256)")
     ap.add_argument("--replays", type=int, default=200)
     ap.add_argument("--layers", type=int, default=0, help="truncate the model (rehearsal only)")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
+    if not 1 <= args.batch <= 256:
+        raise SystemExit(f"--batch must be 1..256, got {args.batch}")
     if not torch.cuda.is_available():
         raise SystemExit("bench_speculative.py needs a CUDA device")
     graft.load_package()
@@ -89,25 +126,13 @@ def main():
     if args.layers:
         cfg.n_layers = args.layers
     w = M.LlamaWeights(cfg, dev)
+    if args.batch > 1:
+        emit(run_batched(M, w, cfg, dev, info, args), args.out)
+        return
     ks = (1, 3, 7)
     runner = M.LlamaRunner(w, batch=1, max_ctx=PROMPT_LEN + GEN_LEN + 32, pdl=True)
     vers = {k: M.LlamaVerifier(runner, draft_len=k) for k in ks}
-
-    # ---- step cost: plain decode and verify at q = 2, 4, 8, whole and split
-    ctx = PROMPT_LEN + GEN_LEN // 2
-    steps = {}
-    for q in (1,) + tuple(k + 1 for k in ks):
-        s = runner.step_struct if q == 1 else vers[q - 1].step_struct
-        fwd = runner.forward if q == 1 else vers[q - 1].forward
-        row = {}
-        for name, mask in (("total_ms", 0), ("gemv_ms", 1), ("attention_ms", 2)):
-            s.skip_mask = mask
-            runner.context_lens.fill_(ctx)
-            (runner.advance if q == 1 else vers[q - 1].advance)()      # metadata of a context-`ctx` step
-            row[name] = median_replay_ms(capture_forward(fwd), runner, ctx + q, args.replays)
-        s.skip_mask = 0
-        row["ms_per_row"] = row["total_ms"] / q
-        steps[q] = row
+    steps = step_costs(runner, vers, "gemv_ms", args.replays)
 
     # ---- plain greedy generation (the reference stream)
     runner.reset()
@@ -173,11 +198,92 @@ def main():
     res = {"metric": "speculative_decode", "model": f"llama-3-8b q4_k_m synthetic, {cfg.n_layers} layers", "batch": 1,
            "prompt": PROMPT_LEN, "generated": GEN_LEN, "replays": args.replays, **info,
            "steps": {str(q): v for q, v in steps.items()}, "plain": plain, "generation": {str(k): v for k, v in gen.items()}}
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out)
+
+
+def run_batched(M, w, cfg, dev, info, args):
+    """--batch B > 1: the same measurements over B sequences with their own prompts and tables"""
+    B = args.batch
+    ks = tuple(k for k in (1, 3, 7) if B > M.MMVQ_MAX_BATCH or B * (k + 1) <= M.MMVQ_MAX_BATCH)
+    linear = "gemv_ms" if B <= M.MMVQ_MAX_BATCH else "linear_ms"
+    # room for a sequence that accepts more than the others to run ahead of the slowest one
+    runner = M.LlamaRunner(w, batch=B, max_ctx=PROMPT_LEN + 2 * GEN_LEN + 32, pdl=True)
+    vers = {k: M.LlamaVerifier(runner, draft_len=k) for k in ks}
+    steps = step_costs(runner, vers, linear, args.replays)
+    for row in steps.values():
+        row["vs_plain"] = row["total_ms"] / steps[1]["total_ms"]
+
+    # every sequence its own prompt in its own table; generation only writes positions >= PROMPT_LEN, so the prompts
+    # stay in the cache across the runs below
+    runner.reset()
+    runner.capture()
+    for v in vers.values():
+        v.capture()
+    pre = M.LlamaPrefill(w, max_tokens=PROMPT_LEN, runner=runner)
+    firsts = []
+    for b in range(B):
+        prompt = [1000 + ((131 + 17 * b + i) % 2048) for i in range(PROMPT_LEN)]
+        firsts.append(int(torch.argmax(pre.forward(prompt, table=runner.tables[b]))))
+
+    def start():
+        runner.reset(PROMPT_LEN)
+        runner.set_tokens(firsts)
+        torch.cuda.synchronize()
+
+    start()
+    ids = torch.zeros(GEN_LEN, B, dtype=torch.int32, device=dev)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(GEN_LEN):
+        runner.graph.replay()
+        ids[i].copy_(runner.meta["token_ids"])
+    e1.record()
+    torch.cuda.synchronize()
+    plain_ids = ids.t().cpu().tolist()
+    plain = {"tok_s_device": B * GEN_LEN / (e0.elapsed_time(e1) / 1e3)}
+    start()
+    tok_h = torch.tensor(firsts, dtype=torch.int32).pin_memory()
+    t0 = time.perf_counter()
+    for _ in range(GEN_LEN):
+        runner.meta["token_ids"].copy_(tok_h, non_blocking=True)
+        runner.graph.replay()
+        tok_h.copy_(runner.meta["token_ids"], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+    plain["tok_s_host_loop"] = B * GEN_LEN / (time.perf_counter() - t0)
+
+    gen = {}
+    for k in ks:
+        gen[k] = {}
+        for target in (1.0, 0.8, 0.5):
+            e = corruption_for(target, k)
+            rng = np.random.default_rng(int(1000 * target) + k)
+            calls = itertools.count()
+
+            def propose(history, k=k, e=e, rng=rng, calls=calls):
+                # speculative_generate asks for the drafts of sequences 0 .. B-1 in order, once per step (two
+                # sequences may share a first token, so that cannot tell them apart)
+                b = next(calls) % B
+                assert history[0] == firsts[b]
+                at = len(history) - 1
+                d = [plain_ids[b][at + i] if at + i < GEN_LEN else 0 for i in range(k)]
+                return [(t + 1) % cfg.vocab if rng.random() < e else t for t in d]
+            start()
+            t0 = time.perf_counter()
+            streams, acc = M.speculative_generate(vers[k], firsts, GEN_LEN, propose)
+            torch.cuda.synchronize()
+            dt = time.perf_counter() - t0
+            a = np.array(acc)
+            mism = {b: next(i for i, (x, y) in enumerate(zip(streams[b], plain_ids[b])) if x != y)
+                    for b in range(B) if streams[b] != plain_ids[b]}
+            gen[k][str(target)] = {"tok_s": B * GEN_LEN / dt, "steps": len(acc), "mean_accepted": float(a.mean()),
+                                   "acceptance": float(a.mean() / k),
+                                   "tokens_per_step": float(1 + a.mean()),
+                                   "streams_equal_plain_greedy": B - len(mism),
+                                   "first_mismatch": {str(b): i for b, i in mism.items()}}
+    return {"metric": "speculative_decode", "model": f"llama-3-8b q4_k_m synthetic, {cfg.n_layers} layers", "batch": B,
+            "route": "gemv" if B <= M.MMVQ_MAX_BATCH else "gemm", "prompt": PROMPT_LEN, "generated": GEN_LEN,
+            "replays": args.replays, **info, "steps": {str(q): v for q, v in steps.items()}, "plain": plain,
+            "generation": {str(k): v for k, v in gen.items()}}
 
 
 if __name__ == "__main__":
