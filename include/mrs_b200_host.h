@@ -104,6 +104,22 @@ int64_t mrs_make_decode_tiles(const int64_t *table_lens, const int64_t *context_
                               int64_t split_pages, int64_t padded_tiles_len, int32_t *request_indices,
                               int32_t *kv_tile_indices, int32_t *o_indptr, int32_t *kv_chunk_size, uint8_t *mask);
 
+/* ---- prompt chunk plan for text prompts (REF pipeline/prompt_chunks.rs, host/prompt_chunks.hpp) ----
+ * mrs_prompt_chunk_size: max(1, budget / batch), each scheduled prompt's share of a step's token budget.
+ * mrs_build_prompt_chunk_plan: rows [prefix_len, total_len) in chunks of at most chunk_size (>= 1); with block_align > 0
+ *   a chunk that would end inside a block ends at that block's start when the chunk stays non-empty.  Writes the chunks
+ *   as [start, end) pairs into out[2 * cap] when they fit; returns their count, -1 on a negative argument.
+ * mrs_next_prompt_chunk_group: n sequences' plans as one CSR (chunks [total][2], plan_offsets [n + 1]) and the index of
+ *   each one's next chunk (plan_indices [n]; past its plan when it has none left).  The first sequence with a chunk
+ *   left sets finality (its plan's last chunk or not) and query length; every sequence with a chunk of the same
+ *   finality (and, with require_uniform_query_len, the same length) is a member.  Writes the members in order to
+ *   members[n] and finality to *is_final; returns the member count, 0 when no chunk is left, -1 on bad arguments. */
+int64_t mrs_prompt_chunk_size(int64_t batch, int64_t budget);
+int64_t mrs_build_prompt_chunk_plan(int64_t total_len, int64_t prefix_len, int64_t chunk_size, int64_t block_align,
+                                    int64_t *out, int64_t cap);
+int64_t mrs_next_prompt_chunk_group(const int64_t *plan_indices, const int64_t *plan_offsets, const int64_t *chunks,
+                                    int64_t n, int32_t require_uniform_query_len, int64_t *members, int32_t *is_final);
+
 /* ---- GGUF archives ---- */
 /* paths: all shards of one model, any order (split.no decides).  NULL + message in err on failure. */
 void *mrs_gguf_open(const char *const *paths, int32_t n_paths, char *err, int64_t err_cap);

@@ -144,6 +144,69 @@ int32_t mrs_spec_accept(const int32_t *argmax, int32_t *token_ids, const int64_t
 int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,
                               int32_t *emitted, void *stream);
 
+/* Batched prompt prefill (REF: the scheduler's prompt step, paged_attention/scheduler.rs, run as one model forward over
+ * the packed rows of every scheduled sequence; `extract_logits`, pipeline/mod.rs, keeps each sequence's last row for the
+ * lm_head): the prompts (or prompt chunks) of n sequences, T rows in all, through the layer stack in one pass.
+ *
+ * One call's plan and buffers.  Row r of every [T, ...] array is a new token of some sequence; sequence i owns rows
+ * cu_seqlens_q[i] .. cu_seqlens_q[i+1] - 1, in order.  All pointers are device pointers unless noted. */
+typedef struct {
+  int32_t n_seqs;              /* n, 1..256 */
+  int32_t total_tokens;        /* T = cu_seqlens_q[n], >= n */
+  int32_t max_q_len;           /* max over i of the new rows of sequence i */
+  int32_t max_kv_len;          /* max over i of cu_seqlens_k[i+1] - cu_seqlens_k[i] (cached + new rows) */
+  int32_t paged;               /* 0: no sequence has cached rows (cu_seqlens_k == cu_seqlens_q): causal attention over the
+                                *    fresh q/k/v, then the KV scatter; 1: the scatter first, then the paged prompt
+                                *    attention over block_tables (prefix-cache hits, later chunks of a chunked prompt) */
+  int32_t lm_rows;             /* 0: no lm_head (a non-final chunk group); 1: each sequence's last row (logits [n, vocab],
+                                *    argmax into out_token); 2: every row (logits [T, vocab], no argmax) */
+  int32_t block_table_stride;  /* entries per row of block_tables (paged) */
+  int32_t num_blocks;          /* blocks in each layer's cache (paged) */
+  const int32_t *token_ids;    /* [T] */
+  const int32_t *positions;    /* [T] RoPE positions (cached + i for the i-th new row of a sequence) */
+  const int64_t *slot_mapping; /* [T] cache slot of each new row (block * block_size + offset) */
+  const int32_t *cu_seqlens_q; /* [n + 1] cumulative new rows */
+  const int32_t *cu_seqlens_k; /* [n + 1] cumulative cached + new rows */
+  const int32_t *block_tables; /* [n, block_table_stride] block ids per sequence (read when paged) */
+  const int32_t *last_rows;    /* [n] row of each sequence's last new token (read when lm_rows == 1) */
+  /* scratch, activation dtype: x, x2 [T, hidden] residual ping-pong, h [T, hidden] normed activations, q [T, n_heads *
+   * head_dim], k, v [T, n_kv_heads * head_dim], attn_out [T, n_heads * head_dim], act [T, inter] */
+  void *x, *x2, *h, *q, *k, *v, *attn_out, *act;
+  void *gate_up;               /* [2, T, inter]: the separate gate and up GEMM outputs; read only when T > 2048 */
+  void *h_last;                /* [n, hidden] the last rows' normed activations (lm_rows == 1) */
+  void *logits;                /* [n, vocab] (lm_rows 1) or [T, vocab] (lm_rows 2) */
+  int32_t *out_token;          /* [n] argmax of each sequence's logits (lm_rows 1) */
+  void *argmax_scratch;        /* zeroed, >= 16 * n + 16 bytes (lm_rows 1); left zeroed */
+  void *q8_scratch;            /* >= n * ceil(hidden / 512) * 16 * 36 bytes: the Q8_1 activations of the n <= 8 lm_head */
+  /* optional commit into a decode runner's rows (lm_rows == 1 only; NULL dest_rows: no commit) */
+  const int32_t *dest_rows;    /* [n] runner row of sequence i */
+  int32_t *runner_token_ids;   /* [runner batch] runner_token_ids[dest_rows[i]] = out_token[i] */
+  int32_t *runner_context_lens;/* [runner batch] runner_context_lens[dest_rows[i]] = cu_seqlens_k[i+1] - cu_seqlens_k[i] */
+} mrs_llama_prefill;
+
+/* Enqueue one prompt step on `stream`: `s` gives weights, norms, per-layer caches, dims, activation dtype, RoPE tables,
+ * rope_neox and pdl (its per-step decode metadata and scratch are not read).  Launches:
+ *   embedding gather over the T rows -> RMSNorm;
+ *   per layer: QKV on the wgmma dequant GEMM (grouped as in the 9..256-sequence decode step: one launch when q, k and v
+ *   share a ggml type, q|k + v when attn_v has its own, else three; above 2048 rows always three, where the grouped
+ *   form measured slower) -> RoPE at `positions` -> attention (paged 0:
+ *   mrs_prefill_attention over cu_seqlens_q, then reshape_and_cache_flashinfer; paged 1: the scatter, then
+ *   mrs_prefill_attention_paged) -> o GEMM -> add + RMSNorm -> gate|up GEMM with the SiLU*mul epilogue (above 2048
+ *   rows: gate and up GEMMs into gate_up, then fused_glu; bit-identical) -> down GEMM
+ *   -> add + RMSNorm with the next layer's norm (the final norm after the last layer);
+ *   lm_rows 1: the last rows gathered into h_last, the lm_head on those n rows by the reference's n-row route (n <= 8:
+ *   Q8_1 quantiser + MMVQ, as `fast_mmvq` plain; n > 8: the dequant GEMM), mrs_argmax into out_token, then the commit
+ *   when dest_rows is set; lm_rows 2: the lm_head GEMM over all T rows.
+ * Each row's GEMMs (never split over K) and norms, and each sequence's attention, are computed on their own: a
+ * sequence's K/V rows do not depend on the other sequences of the call, nor do its logits for a given n-row route.  The GEMMs and norms are links of a PDL chain when s->pdl
+ * is set.  Not graph-capturable in general (T and the max lengths change from call to call).
+ * cudaErrorInvalidValue, before any launch, for: n outside 1..256; T < n; a NULL required pointer (the plan arrays,
+ * x / x2 / h / q / k / v / attn_out / act; gate_up when T > 2048; block_tables, with block_table_stride and num_blocks >= 1, when paged; last_rows, h_last, logits, out_token,
+ * argmax_scratch, and q8_scratch for n <= 8, when lm_rows == 1; logits when lm_rows == 2; runner_token_ids and
+ * runner_context_lens when dest_rows is set); an activation dtype other than f16 / bf16; tensor parallelism (s->tp or
+ * s->all_reduce set); lm_rows outside 0..2; dest_rows set while lm_rows != 1; paged outside 0..1. */
+int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_llama_prefill *p, void *stream);
+
 /* rows of a quantised table -> activation dtype (embedding gather). ids on device. */
 int32_t mrs_embedding_gather(int32_t ggml_type, const void *table, int32_t cols, const int32_t *ids, int32_t n,
                              void *out, int32_t act_dtype, void *stream);

@@ -84,8 +84,10 @@ int32_t mrs_mmq_gguf(int32_t ggml_type, const void *w, const void *x, void *y, i
  * y[0] = T(silu(T(X . W_0^T))) * T(X . W_1^T) with the product rounded in T, as fused_glu.
  * pdl != 0: a link of a programmatic-dependent-launch chain — the weights stream before the upstream grid completes,
  * X is read and Y written after; the launch before it on `stream` must be a link or a plain kernel.
- * dtype 0 f16, 1 bf16; K % 64 == 0 (% 256 for k-quants); w, x 16-byte aligned, y 2-byte aligned.  0 or a cudaError
- * (cudaErrorInvalidValue for a bad type, count or shape, cudaErrorMisalignedAddress).  Kernel: csrc/mmq_tc.cu. */
+ * dtype 0 f16, 1 bf16; K % 64 == 0 (% 256 for k-quants); w, x 16-byte aligned, y 2-byte aligned.  pdl bit 0: PDL
+ * link; bit 1 (value 2): never split K over a cluster, so every output row is the same for any M (a split, chosen from
+ * M, sums the K partials in another order).  0 or a cudaError (cudaErrorInvalidValue for a bad type, count or shape,
+ * cudaErrorMisalignedAddress).  Kernel: csrc/mmq_tc.cu. */
 int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const void **w, const int32_t *rows, void **y,
                              const void *x, int32_t M, int32_t K, int32_t dtype, int32_t glu, int32_t pdl, void *stream);
 

@@ -19,6 +19,8 @@ extern "C" int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, c
 extern "C" int mrs_mmvq_fused_qkv_mixed(int type_qk, int type_v, int dt, const void *wq, const void *wk, const void *wv,
                                         const void *x, const void *norm_w, float eps, void *q, void *k, void *v,
                                         int K, int nq, int nk, int nv, int b_size, int pdl, void *stream);
+extern "C" int32_t mrs_mmq_gguf(int32_t ggml_type, const void *w, const void *x, void *y, int32_t M, int32_t N, int32_t K,
+                                int32_t dtype, void *stream);
 extern "C" int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const void **w, const int32_t *rows,
                                         void **y, const void *x, int32_t M, int32_t K, int32_t dtype, int32_t glu,
                                         int32_t pdl, void *stream);
@@ -67,6 +69,34 @@ extern "C" int32_t flashinfer_decode(void *q, void *key_cache, void *value_cache
                                      int32_t q_stride_h, float sm_scale, int32_t window_left, float logits_soft_cap,
                                      float k_scale, float v_scale, uint32_t dtype, uint32_t cache_dtype,
                                      cudaStream_t stream);
+
+extern "C" int32_t mrs_prefill_attention(const void *q, const void *k, const void *v, void *out, const int32_t *cu_seqlens,
+                                         int32_t batch, int32_t total_tokens, int32_t max_seqlen, int32_t num_heads,
+                                         int32_t num_kv_heads, int32_t head_dim, int64_t q_stride, int64_t kv_stride,
+                                         int64_t o_stride, float softmax_scale, int32_t causal, int32_t window_left,
+                                         float softcap, uint32_t dtype, void *stream);
+extern "C" int32_t mrs_prefill_attention_paged(const void *q, const void *key_cache, const void *value_cache, void *out,
+                                               const int32_t *block_table, int32_t block_table_stride,
+                                               const int32_t *cu_seqlens_q, const int32_t *cu_seqlens_k, int32_t batch,
+                                               int32_t total_q, int32_t max_seqlen_q, int32_t max_seqlen_k, int32_t num_blocks,
+                                               int32_t num_heads, int32_t num_kv_heads, int32_t head_dim, int32_t page_size,
+                                               int64_t q_stride, int64_t o_stride, float softmax_scale, int32_t causal,
+                                               int32_t window_left, float softcap, uint32_t dtype, void *stream);
+extern "C" void fused_glu_f16(const void *a, const void *b, void *output, uint32_t rows, uint32_t cols, uint32_t a_row_stride,
+                              uint32_t b_row_stride, int activation, cudaStream_t stream);
+extern "C" void fused_glu_bf16(const void *a, const void *b, void *output, uint32_t rows, uint32_t cols, uint32_t a_row_stride,
+                               uint32_t b_row_stride, int activation, cudaStream_t stream);
+// the reference-shaped MMVQ launchers (mmvq.cu) the n <= 8 prompt lm_head issues, as `quant.plain` / fast_mmvq plain
+extern "C" void launch_mmvq_gguf_quantize_q8_1_bf16(const void *x, void *vy, int kx, int kx_padded, int num_rows, void *stream);
+extern "C" void launch_mmvq_gguf_quantize_q8_1_f16(const void *x, void *vy, int kx, int kx_padded, int num_rows, void *stream);
+#define MRS_PLAIN_DECL(tag)                                                                                             \
+  extern "C" void launch_mmvq_gguf_##tag##_bf16_plain(const void *vx, const void *vy, void *dst, int ncols_x, int nrows_x, \
+                                                      int stride_col_y, int stride_col_dst, int b_size, void *stream);    \
+  extern "C" void launch_mmvq_gguf_##tag##_f16_plain(const void *vx, const void *vy, void *dst, int ncols_x, int nrows_x,  \
+                                                     int stride_col_y, int stride_col_dst, int b_size, void *stream);
+MRS_PLAIN_DECL(q4_0) MRS_PLAIN_DECL(q4_1) MRS_PLAIN_DECL(q5_0) MRS_PLAIN_DECL(q5_1) MRS_PLAIN_DECL(q8_0)
+MRS_PLAIN_DECL(q2_k) MRS_PLAIN_DECL(q3_k) MRS_PLAIN_DECL(q4_k) MRS_PLAIN_DECL(q5_k) MRS_PLAIN_DECL(q6_k)
+#undef MRS_PLAIN_DECL
 
 namespace mrs {
 
@@ -332,6 +362,26 @@ __global__ void spec_accept_kernel(const int32_t *__restrict__ argmax, int32_t *
   accepted[b] = a;
   context_lens[b] += 1 + a - q;            // the advance left c + q
   row[0] = am[a];
+}
+
+// prompt step: h_last[i] = h[last_rows[i]] (the reference's extract_logits: only each sequence's last row goes through
+// the lm_head).  Grid n, 16-byte copies (hidden * 2 bytes is a multiple of 16).
+__global__ void last_row_gather_kernel(const uint4 *__restrict__ h, const int32_t *__restrict__ last_rows,
+                                       uint4 *__restrict__ h_last, int row_vecs) {
+  const int64_t src = (int64_t)last_rows[blockIdx.x] * row_vecs, dst = (int64_t)blockIdx.x * row_vecs;
+  for (int i = threadIdx.x; i < row_vecs; i += blockDim.x) h_last[dst + i] = h[src + i];
+}
+
+// prompt step hand-off to a decode runner: row dest_rows[i] continues sequence i from its first sampled token, at the
+// context length the prompt step left in the cache
+__global__ void prefill_commit_kernel(const int32_t *__restrict__ out_token, const int32_t *__restrict__ cu_k,
+                                      const int32_t *__restrict__ dest_rows, int32_t *__restrict__ token_ids,
+                                      int32_t *__restrict__ context_lens, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int r = dest_rows[i];
+  token_ids[r] = out_token[i];
+  context_lens[r] = cu_k[i + 1] - cu_k[i];
 }
 
 }  // namespace mrs
@@ -690,4 +740,143 @@ extern "C" int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len,
   MRS_TRY(gemm ? llama_forward_gemm(s, q_len, stream) : llama_forward(s, q_len, stream));
   return mrs_spec_accept(s->out_token, s->token_ids, s->slot_mapping, context_lens, accepted, emitted, s->batch, q_len,
                          s->pdl, stream);
+}
+
+// Above this many rows the prompt step runs q, k and v as separate GEMMs, and gate and up as two GEMMs + fused_glu,
+// instead of the grouped launches.  Measured on an H100 SXM (700 W), Llama-3-8B layer shapes (DESIGN §5.3): the
+// grouped QKV takes 0.54-0.89 x the separate launches from 256 to 2048 rows on Q8_0 but 1.17 x at 4096 and 1.12 x at
+// 8192 (Q4_K_M's q|k + v: 0.89 x at 256 rows, 1.09-1.15 x from 1024 up); the GLU epilogue takes 0.93-0.94 x at 1024
+// rows and 1.00-1.03 x from 2048 up.  Results are bit-identical either way.
+constexpr int PREFILL_GROUPED_MAX_ROWS = 2048;
+
+// the prompt step over the packed rows of n sequences (contract: include/mrs_b200_model.h).  The layer chain is the one
+// of llama_forward_gemm over T rows; attention is the var-len prompt attention instead of the decode attention.
+extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_llama_prefill *p, void *stream) {
+  if (s == nullptr || p == nullptr) return (int32_t)cudaErrorInvalidValue;
+  const int n = p->n_seqs, T = p->total_tokens, dt = s->act_dtype, H = s->hidden, pdl = s->pdl;
+  if (n < 1 || n > 256 || T < n || (dt != MRS_F16 && dt != MRS_BF16) || s->tp != nullptr || s->all_reduce != nullptr ||
+      p->lm_rows < 0 || p->lm_rows > 2 || (p->paged != 0 && p->paged != 1) || (p->dest_rows != nullptr && p->lm_rows != 1) ||
+      p->max_q_len < 1 || p->max_kv_len < p->max_q_len || H % 8 != 0)
+    return (int32_t)cudaErrorInvalidValue;
+  if (s->layers == nullptr || p->token_ids == nullptr || p->positions == nullptr || p->slot_mapping == nullptr ||
+      p->cu_seqlens_q == nullptr || p->cu_seqlens_k == nullptr || p->x == nullptr || p->x2 == nullptr || p->h == nullptr ||
+      p->q == nullptr || p->k == nullptr || p->v == nullptr || p->attn_out == nullptr || p->act == nullptr)
+    return (int32_t)cudaErrorInvalidValue;
+  const bool grouped = T <= PREFILL_GROUPED_MAX_ROWS;
+  if (!grouped && p->gate_up == nullptr) return (int32_t)cudaErrorInvalidValue;
+  if (p->paged && (p->block_tables == nullptr || p->block_table_stride < 1 || p->num_blocks < 1)) return (int32_t)cudaErrorInvalidValue;
+  if (p->lm_rows == 1 && (p->last_rows == nullptr || p->h_last == nullptr || p->logits == nullptr || p->out_token == nullptr ||
+                          p->argmax_scratch == nullptr || (n <= 8 && p->q8_scratch == nullptr)))
+    return (int32_t)cudaErrorInvalidValue;
+  if (p->lm_rows == 2 && p->logits == nullptr) return (int32_t)cudaErrorInvalidValue;
+  if (p->dest_rows != nullptr && (p->runner_token_ids == nullptr || p->runner_context_lens == nullptr))
+    return (int32_t)cudaErrorInvalidValue;
+
+  const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
+  cudaStream_t st = (cudaStream_t)stream;
+  // pdl | 2: K is never split, so a sequence's rows come out the same whatever other rows share the launch
+  auto gemm = [&](int type, int nm, const void **w, const int32_t *rows, void **y, const void *x, int M, int K, int glu) {
+    return mrs_mmq_gguf_grouped(type, nm, w, rows, y, x, M, K, dt, glu, pdl | 2, stream);
+  };
+  // one matrix: above 64 rows the plain ggml source of mrs_mmq_gguf, which runs faster than the grouped source at
+  // prefill sizes and never splits K there (tc_gemm.cuh splits only token tiles of up to 64 rows); up to 64 rows the
+  // grouped launch with whole K.  Same results either way.
+  auto linear = [&](const mrs_qweight &W, int N, void *y, const void *x, int M, int K) -> int32_t {
+    if (M > 64) return mrs_mmq_gguf(W.ggml_type, W.data, x, y, M, N, K, dt, stream);
+    const void *w[1] = {W.data};
+    const int32_t rows[1] = {N};
+    void *yy[1] = {y};
+    return gemm(W.ggml_type, 1, w, rows, yy, x, M, K, 0);
+  };
+  auto add_rms = [&](const void *x, const void *res, const void *w, void *res_dst) {
+    mrs_add_rms_norm_pdl(x, res, w, res_dst, p->h, T, H, s->rms_eps, dt, pdl, stream);
+  };
+
+  MRS_TRY(mrs_embedding_gather(s->tok_embd.ggml_type, s->tok_embd.data, H, p->token_ids, T, p->x, dt, stream));
+  if (dt == MRS_F16) mrs_rms_norm_f16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
+  else mrs_rms_norm_bf16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
+  for (int l = 0; l < s->n_layers; l++) {
+    const mrs_llama_layer &L = s->layers[l];
+    {
+      const void *w[3] = {L.wq.data, L.wk.data, L.wv.data};
+      int32_t rows[3] = {nq, nkv, nkv};
+      void *y[3] = {p->q, p->k, p->v};
+      if (grouped && L.wq.ggml_type == L.wk.ggml_type && L.wk.ggml_type == L.wv.ggml_type) {
+        MRS_TRY(gemm(L.wq.ggml_type, 3, w, rows, y, p->h, T, H, 0));
+      } else if (grouped && L.wq.ggml_type == L.wk.ggml_type) {   // Q4_K_M keeps attn_v in Q6_K on some layers
+        MRS_TRY(gemm(L.wq.ggml_type, 2, w, rows, y, p->h, T, H, 0));
+        MRS_TRY(linear(L.wv, nkv, p->v, p->h, T, H));
+      } else {
+        MRS_TRY(linear(L.wq, nq, p->q, p->h, T, H));
+        MRS_TRY(linear(L.wk, nkv, p->k, p->h, T, H));
+        MRS_TRY(linear(L.wv, nkv, p->v, p->h, T, H));
+      }
+    }
+    rotary_embedding_positions(p->q, p->k, (void *)s->rope_cos, (void *)s->rope_sin, (void *)p->positions, s->rope_neox,
+                               s->head_dim, T, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt,
+                               (int64_t)stream);
+    if (!p->paged) {   // every key is new: attend over the fresh rows, then write them to the cache
+      MRS_TRY(mrs_prefill_attention(p->q, p->k, p->v, p->attn_out, p->cu_seqlens_q, n, T, p->max_q_len, s->n_heads,
+                                    s->n_kv_heads, s->head_dim, nq, nkv, nq, s->sm_scale, 1, -1, 0.f, (uint32_t)dt, stream));
+      reshape_and_cache_flashinfer(p->k, p->v, L.k_cache, L.v_cache, (int64_t *)p->slot_mapping, T, s->n_kv_heads,
+                                   s->head_dim, s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
+    } else {           // the new rows join the cached ones in the cache, then attend over the pages
+      reshape_and_cache_flashinfer(p->k, p->v, L.k_cache, L.v_cache, (int64_t *)p->slot_mapping, T, s->n_kv_heads,
+                                   s->head_dim, s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
+      MRS_TRY(mrs_prefill_attention_paged(p->q, L.k_cache, L.v_cache, p->attn_out, p->block_tables, p->block_table_stride,
+                                          p->cu_seqlens_q, p->cu_seqlens_k, n, T, p->max_q_len, p->max_kv_len,
+                                          p->num_blocks, s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, nq, nq,
+                                          s->sm_scale, 1, -1, 0.f, (uint32_t)dt, stream));
+    }
+    MRS_TRY(linear(L.wo, H, p->h, p->attn_out, T, nq));
+    add_rms(p->h, p->x, L.ffn_norm, p->x2);                                     // x2 = o + x ; h = norm(x2)
+    if (L.w_gate.ggml_type != L.w_up.ggml_type || L.w_gate.rows != L.w_up.rows) return (int32_t)cudaErrorInvalidValue;
+    if (grouped) {
+      const void *w[2] = {L.w_gate.data, L.w_up.data};
+      const int32_t rows[2] = {L.w_gate.rows, L.w_up.rows};
+      void *y[2] = {p->act, nullptr};
+      MRS_TRY(gemm(L.w_gate.ggml_type, 2, w, rows, y, p->h, T, H, 1));
+    } else {   // gate and up into the two halves of gate_up, then SiLU(gate) * up
+      const int I = L.w_gate.rows;
+      void *up = (uint8_t *)p->gate_up + (size_t)T * I * 2;
+      MRS_TRY(linear(L.w_gate, I, p->gate_up, p->h, T, H));
+      MRS_TRY(linear(L.w_up, I, up, p->h, T, H));
+      if (dt == MRS_F16) fused_glu_f16(p->gate_up, up, p->act, T, I, I, I, 0, st);
+      else fused_glu_bf16(p->gate_up, up, p->act, T, I, I, I, 0, st);
+    }
+    MRS_TRY(linear(L.w_down, H, p->h, p->act, T, L.w_down.cols));
+    add_rms(p->h, p->x2, l + 1 < s->n_layers ? s->layers[l + 1].attn_norm : s->final_norm, p->x);   // x = down + x2 ; h = next norm(x)
+  }
+  if (p->lm_rows == 2) {
+    MRS_TRY(linear(s->lm_head, s->vocab, p->logits, p->h, T, H));
+  } else if (p->lm_rows == 1) {
+    last_row_gather_kernel<<<n, 128, 0, st>>>((const uint4 *)p->h, p->last_rows, (uint4 *)p->h_last, H / 8);
+    if (n <= 8) {    // the reference's GgufMatMul at 1..8 rows: Q8_1 activations + MMVQ (fast_mmvq plain)
+      const int kpad = (H + 511) / 512 * 512;
+      if (dt == MRS_F16) launch_mmvq_gguf_quantize_q8_1_f16(p->h_last, p->q8_scratch, H, kpad, n, stream);
+      else launch_mmvq_gguf_quantize_q8_1_bf16(p->h_last, p->q8_scratch, H, kpad, n, stream);
+      const void *W = s->lm_head.data;
+      const int V = s->vocab, sy = kpad / 32;
+#define MRS_PLAIN_CASE(TYPE, tag)                                                                        \
+  case TYPE:                                                                                             \
+    if (dt == MRS_F16) launch_mmvq_gguf_##tag##_f16_plain(W, p->q8_scratch, p->logits, H, V, sy, V, n, stream); \
+    else launch_mmvq_gguf_##tag##_bf16_plain(W, p->q8_scratch, p->logits, H, V, sy, V, n, stream);            \
+    break;
+      switch (s->lm_head.ggml_type) {
+        MRS_PLAIN_CASE(MRS_Q4_0, q4_0) MRS_PLAIN_CASE(MRS_Q4_1, q4_1) MRS_PLAIN_CASE(MRS_Q5_0, q5_0)
+        MRS_PLAIN_CASE(MRS_Q5_1, q5_1) MRS_PLAIN_CASE(MRS_Q8_0, q8_0) MRS_PLAIN_CASE(MRS_Q2_K, q2_k)
+        MRS_PLAIN_CASE(MRS_Q3_K, q3_k) MRS_PLAIN_CASE(MRS_Q4_K, q4_k) MRS_PLAIN_CASE(MRS_Q5_K, q5_k)
+        MRS_PLAIN_CASE(MRS_Q6_K, q6_k)
+        default: return (int32_t)cudaErrorInvalidValue;
+      }
+#undef MRS_PLAIN_CASE
+    } else {         // 9 and more rows: the dequant GEMM (the reference's MMQ branch)
+      MRS_TRY(linear(s->lm_head, s->vocab, p->logits, p->h_last, n, H));
+    }
+    MRS_TRY(mrs_argmax(p->logits, n, s->vocab, dt, p->out_token, p->argmax_scratch, pdl, stream));
+    if (p->dest_rows != nullptr)
+      prefill_commit_kernel<<<(n + 127) / 128, 128, 0, st>>>(p->out_token, p->cu_seqlens_k, p->dest_rows,
+                                                             p->runner_token_ids, p->runner_context_lens, n);
+  }
+  return (int32_t)cudaGetLastError();
 }

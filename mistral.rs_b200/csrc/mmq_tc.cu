@@ -277,10 +277,10 @@ extern "C" int32_t mrs_mmq_gguf(int32_t ggml_type, const void *w, const void *x,
 
 template <bool GLU>
 static cudaError_t mmq_group_run(int type, const GgmlGroupSrc<MRS_Q4_0, GLU> &a, const void *x, int M, int N, int K, int dtype,
-                                 int pdl, cudaStream_t st) {
+                                 int pdl, bool split_k, cudaStream_t st) {
   // one field layout for every type: only the decoder differs
 #define MRS_GG(T) return hg_run(GgmlGroupSrc<T, GLU>{a.w0, a.w1, a.w2, a.y0, a.y1, a.y2, a.r0, a.r1, a.r2, a.row_bytes, a.bf}, \
-                                x, nullptr, nullptr, M, N, K, dtype, pdl, st)
+                                x, nullptr, nullptr, M, N, K, dtype, pdl, st, split_k)
   switch (type) {
   case MRS_Q4_0: MRS_GG(MRS_Q4_0);
   case MRS_Q4_1: MRS_GG(MRS_Q4_1);
@@ -306,6 +306,8 @@ extern "C" int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const
                                         void **y, const void *x, int32_t M, int32_t K, int32_t dtype, int32_t glu,
                                         int32_t pdl, void *stream) {
   if (n_mats < 1 || n_mats > 3 || w == nullptr || rows == nullptr || y == nullptr) return (int32_t)cudaErrorInvalidValue;
+  const bool split_k = !(pdl & 2);
+  pdl &= 1;
   if (glu && (n_mats != 2 || rows[0] != rows[1])) return (int32_t)cudaErrorInvalidValue;
   if (M <= 0) return 0;
   const int rb = tc_row_bytes(ggml_type, K);
@@ -326,9 +328,9 @@ extern "C" int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const
   cudaStream_t st = (cudaStream_t)stream;
   if (glu) {
     const GgmlGroupSrc<MRS_Q4_0, true> g{a.w0, a.w1, nullptr, a.y0, a.y1, nullptr, a.r0, a.r1, 0, rb, dtype};
-    return (int32_t)mmq_group_run<true>(ggml_type, g, x, M, (rows[0] + 63) / 64 * HG_BM, K, dtype, pdl, st);
+    return (int32_t)mmq_group_run<true>(ggml_type, g, x, M, (rows[0] + 63) / 64 * HG_BM, K, dtype, pdl, split_k, st);
   }
-  return (int32_t)mmq_group_run<false>(ggml_type, a, x, M, (int)total, K, dtype, pdl, st);
+  return (int32_t)mmq_group_run<false>(ggml_type, a, x, M, (int)total, K, dtype, pdl, split_k, st);
 }
 
 // GPTQ / AWQ int4 linear on the tensor cores, straight from the checkpoint tensors (no Marlin

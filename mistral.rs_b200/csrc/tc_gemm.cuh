@@ -296,9 +296,11 @@ static inline int hg_pick_ksplit(int N, int K, int M, int NT) {
 
 // one launch over all token tiles: grid (token tiles, K splits, row tiles), clusters along the K splits.  Token tiles
 // run fastest, so the CTAs that read the same weight rows are resident together and share them through L2.
+// split_k false: one CTA per tile over all of K, so a row's result does not depend on M (the K split does)
 template <class Src, int NT, bool BF>
-static cudaError_t hg_launch_nt(const CUtensorMap &tx, const CUtensorMap &tw, const Src &src, HgShape p, cudaStream_t st) {
-  const int ks = hg_pick_ksplit(p.N, p.K, p.M, NT);
+static cudaError_t hg_launch_nt(const CUtensorMap &tx, const CUtensorMap &tw, const Src &src, HgShape p, cudaStream_t st,
+                                bool split_k) {
+  const int ks = split_k ? hg_pick_ksplit(p.N, p.K, p.M, NT) : 1;
   const int nk = p.K / HG_BK;
   p.ksteps_per_split = (nk + ks - 1) / ks;
   const size_t smem = hg_smem_bytes(NT, ks);
@@ -328,7 +330,8 @@ static cudaError_t hg_launch_nt(const CUtensorMap &tx, const CUtensorMap &tw, co
 
 // x: [M, K] 16-bit row-major (dtype 0 f16, 1 bf16); w_dense: [N, K] when Src::kTmaA.  K % 64 == 0.
 template <class Src>
-static cudaError_t hg_run(const Src &src, const void *x, const void *w_dense, void *y, int M, int N, int K, int dtype, int pdl, cudaStream_t st) {
+static cudaError_t hg_run(const Src &src, const void *x, const void *w_dense, void *y, int M, int N, int K, int dtype, int pdl, cudaStream_t st,
+                          bool split_k = true) {
   if (M <= 0 || N <= 0) return cudaSuccess;
   if (K % HG_BK != 0 || (dtype != MRS_F16 && dtype != MRS_BF16)) return cudaErrorInvalidValue;
   const int NT = M <= 32 ? 32 : M <= 64 ? 64 : M <= 128 ? 128 : 256;
@@ -341,7 +344,7 @@ static cudaError_t hg_run(const Src &src, const void *x, const void *w_dense, vo
   }
   HgShape p = {y, M, N, K, 0, pdl};
   const bool bf = dtype == MRS_BF16;
-#define MRS_HG(NTV) return bf ? hg_launch_nt<Src, NTV, true>(tx, tw, src, p, st) : hg_launch_nt<Src, NTV, false>(tx, tw, src, p, st)
+#define MRS_HG(NTV) return bf ? hg_launch_nt<Src, NTV, true>(tx, tw, src, p, st, split_k) : hg_launch_nt<Src, NTV, false>(tx, tw, src, p, st, split_k)
   if (NT == 32) MRS_HG(32);
   if (NT == 64) MRS_HG(64);
   if (NT == 128) MRS_HG(128);

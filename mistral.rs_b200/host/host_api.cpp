@@ -3,6 +3,7 @@
 #include "gguf_reader.hpp"
 #include "kv_cache_manager.hpp"
 #include "kv_index.hpp"
+#include "prompt_chunks.hpp"
 #include "safetensors_reader.hpp"
 #include "sampler_tail.hpp"
 
@@ -199,6 +200,41 @@ int64_t mrs_decode_split_pages(int64_t block_size, int64_t batch, int64_t kv_hea
 }
 
 // returns number of valid tiles, or -1 on error
+int64_t mrs_prompt_chunk_size(int64_t batch, int64_t budget) {
+  if (batch < 0 || budget < 0) return -1;
+  return (int64_t)prompt_chunk_size((size_t)batch, (size_t)budget);
+}
+
+int64_t mrs_build_prompt_chunk_plan(int64_t total_len, int64_t prefix_len, int64_t chunk_size, int64_t block_align,
+                                    int64_t *out, int64_t cap) {
+  if (total_len < 0 || prefix_len < 0 || chunk_size < 1 || block_align < 0 || cap < 0) return -1;
+  const auto plan = build_prompt_chunk_plan((size_t)total_len, (size_t)prefix_len, (size_t)chunk_size, (size_t)block_align);
+  if ((int64_t)plan.size() <= cap && out != nullptr)
+    for (size_t i = 0; i < plan.size(); i++) { out[2 * i] = (int64_t)plan[i].start; out[2 * i + 1] = (int64_t)plan[i].end; }
+  return (int64_t)plan.size();
+}
+
+int64_t mrs_next_prompt_chunk_group(const int64_t *plan_indices, const int64_t *plan_offsets, const int64_t *chunks,
+                                    int64_t n, int32_t require_uniform_query_len, int64_t *members, int32_t *is_final) {
+  if (n < 0 || (n > 0 && (plan_indices == nullptr || plan_offsets == nullptr || members == nullptr)) || is_final == nullptr)
+    return -1;
+  std::vector<size_t> idx((size_t)n);
+  std::vector<std::vector<PromptChunk>> plans((size_t)n);
+  for (int64_t i = 0; i < n; i++) {
+    if (plan_indices[i] < 0 || plan_offsets[i + 1] < plan_offsets[i] || (plan_offsets[i + 1] > plan_offsets[i] && chunks == nullptr))
+      return -1;
+    idx[(size_t)i] = (size_t)plan_indices[i];
+    for (int64_t c = plan_offsets[i]; c < plan_offsets[i + 1]; c++)
+      plans[(size_t)i].push_back({(size_t)chunks[2 * c], (size_t)chunks[2 * c + 1]});
+  }
+  std::vector<size_t> m;
+  bool fin = false;
+  if (!next_prompt_chunk_group(idx, plans, require_uniform_query_len != 0, m, fin)) { *is_final = 0; return 0; }
+  for (size_t i = 0; i < m.size(); i++) members[i] = (int64_t)m[i];
+  *is_final = fin ? 1 : 0;
+  return (int64_t)m.size();
+}
+
 int64_t mrs_make_decode_tiles(const int64_t *table_lens, const int64_t *context_lens, int64_t batch, int64_t block_size,
                               int64_t split_pages, int64_t padded_tiles_len, int32_t *request_indices,
                               int32_t *kv_tile_indices, int32_t *o_indptr, int32_t *kv_chunk_size, uint8_t *mask) {

@@ -35,6 +35,8 @@ def host_lib():
             getattr(L, f"mrs_kv_manager_{f}").restype = ctypes.c_int64
         L.mrs_decode_split_pages.restype = ctypes.c_int64
         L.mrs_make_decode_tiles.restype = ctypes.c_int64
+        for f in ("prompt_chunk_size", "build_prompt_chunk_plan", "next_prompt_chunk_group"):
+            getattr(L, f"mrs_{f}").restype = ctypes.c_int64
         _lib = L
     return _lib
 
@@ -324,3 +326,49 @@ def make_paged_kv_decode_tensors(tables, context_lens, block_size, split_pages, 
     if n < 0:
         raise IndexError("paged kv decode tiles exceed padded length / table too small")
     return req[:padded_tiles_len], tile[:padded_tiles_len], o_indptr, chunk, mask[:padded_tiles_len]
+
+
+# ---- prompt chunk plan (host/prompt_chunks.hpp; REF pipeline/prompt_chunks.rs for text prompts) ----
+def prompt_chunk_size(batch, budget):
+    """Each of `batch` scheduled prompts' share of a step's token budget: max(1, budget // batch)."""
+    r = host_lib().mrs_prompt_chunk_size(ctypes.c_int64(int(batch)), ctypes.c_int64(int(budget)))
+    if r < 0:
+        raise ValueError(f"prompt_chunk_size: need batch, budget >= 0, got {batch}, {budget}")
+    return int(r)
+
+
+def build_prompt_chunk_plan(total_len, prefix_len, chunk_size, block_align=None):
+    """[(start, end)] chunks of rows [prefix_len, total_len), each at most chunk_size; with block_align a chunk that
+    would end inside a block ends at that block's start when it stays non-empty."""
+    args = [int(total_len), int(prefix_len), int(chunk_size), int(block_align or 0)]
+    f = host_lib().mrs_build_prompt_chunk_plan
+    n = f(*[ctypes.c_int64(a) for a in args], None, ctypes.c_int64(0))
+    if n < 0:
+        raise ValueError(f"build_prompt_chunk_plan: bad arguments {args}")
+    out = np.empty(max(1, 2 * n), dtype=np.int64)
+    f(*[ctypes.c_int64(a) for a in args], ctypes.c_void_p(out.ctypes.data), ctypes.c_int64(n))
+    return [(int(out[2 * i]), int(out[2 * i + 1])) for i in range(n)]
+
+
+def next_prompt_chunk_group(plan_indices, plans, require_uniform_query_len=False):
+    """(members, is_final) of the next prompt step, or None when no sequence has a chunk left.  plan_indices[i] is the
+    index of sequence i's next chunk in plans[i] (a list of (start, end)).  The first sequence with a chunk left sets
+    finality and query length; members are the sequences whose next chunk has the same finality (and, with
+    require_uniform_query_len, the same length)."""
+    n = len(plans)
+    if len(plan_indices) != n:
+        raise ValueError(f"next_prompt_chunk_group: {len(plan_indices)} indices for {n} plans")
+    idx = _i64([int(i) for i in plan_indices] or [0])
+    offs = _i64(np.cumsum([0] + [len(p) for p in plans]))
+    flat = _i64([v for p in plans for c in p for v in c] or [0])
+    members = np.empty(max(1, n), dtype=np.int64)
+    fin = ctypes.c_int32(0)
+    r = host_lib().mrs_next_prompt_chunk_group(ctypes.c_void_p(idx.ctypes.data), ctypes.c_void_p(offs.ctypes.data),
+                                               ctypes.c_void_p(flat.ctypes.data), ctypes.c_int64(n),
+                                               ctypes.c_int32(int(bool(require_uniform_query_len))),
+                                               ctypes.c_void_p(members.ctypes.data), ctypes.byref(fin))
+    if r < 0:
+        raise ValueError("next_prompt_chunk_group: bad arguments")
+    if r == 0:
+        return None
+    return [int(m) for m in members[:r]], bool(fin.value)

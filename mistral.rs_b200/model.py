@@ -570,26 +570,7 @@ class LlamaRunner:
                         h=a(batch, H))
         self.k_cache = [a(nb, self.n_kv, bs, cfg.head_dim) for _ in range(cfg.n_layers)]
         self.v_cache = [a(nb, self.n_kv, bs, cfg.head_dim) for _ in range(cfg.n_layers)]
-        self._layers = (_Layer * cfg.n_layers)()
-        for l, L in enumerate(weights.layers):
-            for field_, name in (("wq", "attn_q"), ("wk", "attn_k"), ("wv", "attn_v"), ("wo", "attn_output"),
-                                 ("w_gate", "ffn_gate"), ("w_up", "ffn_up"), ("w_down", "ffn_down")):
-                t, ty, rows, cols = L[name]
-                setattr(self._layers[l], field_, _QW(t.data_ptr(), GGML[ty], rows, cols))
-            self._layers[l].attn_norm = L["attn_norm"].data_ptr()
-            self._layers[l].ffn_norm = L["ffn_norm"].data_ptr()
-            self._layers[l].k_cache = self.k_cache[l].data_ptr()
-            self._layers[l].v_cache = self.v_cache[l].data_ptr()
-        s = _Step()
-        s.hidden, s.n_layers, s.n_heads, s.n_kv_heads, s.head_dim, s.vocab = H, cfg.n_layers, self.n_heads, self.n_kv, cfg.head_dim, cfg.vocab
-        s.block_size, s.act_dtype = bs, {torch.float16: 0, torch.bfloat16: 1}[dt]
-        s.rms_eps, s.sm_scale, s.rope_neox, s.pdl = cfg.rms_eps, 1.0 / float(np.sqrt(cfg.head_dim)), int(cfg.rope_neox), int(pdl)
-        s.layers = ctypes.cast(self._layers, ctypes.POINTER(_Layer))
-        t, ty, rows, cols = weights.tok_embd
-        s.tok_embd = _QW(t.data_ptr(), GGML[ty], rows, cols)
-        t, ty, rows, cols = weights.output
-        s.lm_head = _QW(t.data_ptr(), GGML[ty], rows, cols)
-        s.final_norm, s.rope_cos, s.rope_sin = weights.output_norm.data_ptr(), weights.rope_cos.data_ptr(), weights.rope_sin.data_ptr()
+        self._layers, s = _model_step(weights, self.k_cache, self.v_cache, pdl, self.n_heads, self.n_kv)
         s.batch, s.padded_tiles, s.max_blocks_per_seq = batch, self.padded_tiles, self.max_blocks
         s.fused_attention = int(fused_attention)
         for n, t in self.meta.items():
@@ -679,19 +660,59 @@ class LlamaRunner:
         return self.buf["logits"]
 
 
-class LlamaPrefill:
-    """Prompt processing (one sequence, positions 0..T-1) composed from the C-ABI ops, in the order
-    of the reference's prefill forward (`models/llama.rs` Block::forward with seq_len > 1):
-    RMSNorm -> wgmma dequant-GEMMs (`mmq.forward`, the `fast_mmq` path) -> RoPE -> causal prompt
-    attention over the fresh q/k/v (`paged_attn.prefill_attention`, the reference's flash-attn call,
-    paged_attention.rs:1413-1475) -> KV scatter into the paged HND cache -> o_proj -> add+RMSNorm ->
-    GLU -> down -> add.  TTFT of BASELINE config 3 is the time of `forward` on a 4096-token prompt.
-    `forward(cached=n)` continues a sequence whose first n tokens are already in the cache (prefix-cache hit or
-    chunked prefill): KV scatter first, then paged prompt attention over the cache (`prefill_attention_paged`)."""
+MAX_PREFILL_SEQS = 256   # sequences per prompt step (mrs_llama_prefill_step)
+PREFILL_GROUPED_MAX_ROWS = 2048   # above: separate QKV and gate / up GEMMs (needs the gate_up scratch)
 
-    def __init__(self, weights: "LlamaWeights", max_tokens=4096, runner: "LlamaRunner" = None):
-        """runner: write the prompt's K/V into sequence 0 of this decode runner's paged cache (its block
-        table), so a generation is prefill -> `runner.reset(T)` -> decode-graph replays."""
+
+class _Prefill(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("n_seqs", "total_tokens", "max_q_len", "max_kv_len", "paged", "lm_rows",
+                                              "block_table_stride", "num_blocks")] + \
+               [(n, ctypes.c_void_p) for n in ("token_ids", "positions", "slot_mapping", "cu_seqlens_q", "cu_seqlens_k",
+                                               "block_tables", "last_rows", "x", "x2", "h", "q", "k", "v", "attn_out", "act",
+                                               "gate_up", "h_last", "logits", "out_token", "argmax_scratch", "q8_scratch", "dest_rows",
+                                               "runner_token_ids", "runner_context_lens")]
+
+
+def _model_step(weights, k_cache, v_cache, pdl, n_heads, n_kv_heads):
+    """(layer array, mrs_llama_step) with the model fields only: weights, norms, caches, dims (local head counts under
+    tensor parallelism), RoPE tables; no per-step metadata or scratch.  The layer array must outlive the struct's use."""
+    cfg = weights.cfg
+    layers = (_Layer * cfg.n_layers)()
+    for l, L in enumerate(weights.layers):
+        for field_, name in (("wq", "attn_q"), ("wk", "attn_k"), ("wv", "attn_v"), ("wo", "attn_output"),
+                             ("w_gate", "ffn_gate"), ("w_up", "ffn_up"), ("w_down", "ffn_down")):
+            t, ty, rows, cols = L[name]
+            setattr(layers[l], field_, _QW(t.data_ptr(), GGML[ty], rows, cols))
+        layers[l].attn_norm, layers[l].ffn_norm = L["attn_norm"].data_ptr(), L["ffn_norm"].data_ptr()
+        layers[l].k_cache, layers[l].v_cache = k_cache[l].data_ptr(), v_cache[l].data_ptr()
+    s = _Step()
+    s.hidden, s.n_layers, s.n_heads, s.n_kv_heads, s.head_dim, s.vocab = (cfg.hidden, cfg.n_layers, n_heads, n_kv_heads,
+                                                                          cfg.head_dim, cfg.vocab)
+    s.block_size, s.act_dtype = cfg.block_size, {torch.float16: 0, torch.bfloat16: 1}[weights.dtype]
+    s.rms_eps, s.sm_scale, s.rope_neox, s.pdl = cfg.rms_eps, 1.0 / float(np.sqrt(cfg.head_dim)), int(cfg.rope_neox), int(pdl)
+    s.layers = ctypes.cast(layers, ctypes.POINTER(_Layer))
+    for field_, (t, ty, rows, cols) in (("tok_embd", weights.tok_embd), ("lm_head", weights.output)):
+        setattr(s, field_, _QW(t.data_ptr(), GGML[ty], rows, cols))
+    s.final_norm, s.rope_cos, s.rope_sin = weights.output_norm.data_ptr(), weights.rope_cos.data_ptr(), weights.rope_sin.data_ptr()
+    return layers, s
+
+
+class LlamaPrefill:
+    """Prompt processing through `mrs_llama_prefill_step` (include/mrs_b200_model.h), the reference's prompt forward
+    (`models/llama.rs` Block::forward with seq_len > 1) over the packed rows of one or many sequences:
+    embedding -> per layer RMSNorm, wgmma dequant-GEMMs (grouped QKV, gate|up with the GLU epilogue), RoPE, var-len
+    causal prompt attention over the fresh q/k/v (the reference's flash-attn call, paged_attention.rs:1413-1475) and the
+    KV scatter into the paged HND cache, o_proj, add+RMSNorm, down, add+RMSNorm -> lm_head on each sequence's last row
+    (`extract_logits`) -> argmax.  A sequence with cached rows (prefix-cache hit, or a later chunk of a chunked prompt)
+    has its new K/V scattered first and attends over the cache (`prefill_attention_paged`).
+    `forward` is the one-sequence call; TTFT of BASELINE config 3 is its time on a 4096-token prompt.  `forward_batch`
+    runs up to 256 sequences in one step and can hand them to a decode runner's rows on the device."""
+
+    def __init__(self, weights: "LlamaWeights", max_tokens=4096, runner: "LlamaRunner" = None, pdl=True):
+        """max_tokens: new rows per call (all sequences together); the scratch for them is allocated here.
+        runner: write prompts' K/V into this decode runner's paged cache (sequence 0's block table by default), so a
+        generation is prefill -> `runner.reset(T)` -> decode-graph replays, or `forward_batch(slots=...)` ->
+        decode-graph replays."""
         from . import ops, paged_attn, quant  # noqa: F401  (fail early when the extension is missing)
         cfg, dev, dt = weights.cfg, weights.device, weights.dtype
         if weights.tp_size != 1:
@@ -700,6 +721,7 @@ class LlamaPrefill:
         bs = cfg.block_size
         self.max_tokens = int(max_tokens)
         self.nblocks = -(-self.max_tokens // bs)
+        self.runner = runner
         if runner is not None:
             if runner.max_blocks < self.nblocks:
                 raise ValueError("LlamaPrefill: the runner's block table is shorter than max_tokens")
@@ -709,7 +731,18 @@ class LlamaPrefill:
             self.table = list(range(1, self.nblocks + 1))
             self.k_cache = [torch.zeros(nb, cfg.n_kv_heads, bs, cfg.head_dim, dtype=dt, device=dev) for _ in range(cfg.n_layers)]
             self.v_cache = [torch.zeros(nb, cfg.n_kv_heads, bs, cfg.head_dim, dtype=dt, device=dev) for _ in range(cfg.n_layers)]
-        self._slots = torch.tensor([self.table[i // bs] * bs + i % bs for i in range(self.max_tokens)], dtype=torch.int64, device=dev)
+        T, H = self.max_tokens, cfg.hidden
+        nq, nkv = cfg.n_heads * cfg.head_dim, cfg.n_kv_heads * cfg.head_dim
+        a = lambda *s: torch.empty(*s, dtype=dt, device=dev)
+        self.buf = dict(x=a(T, H), x2=a(T, H), h=a(T, H), q=a(T, nq), k=a(T, nkv), v=a(T, nkv), attn_out=a(T, nq),
+                        act=a(T, cfg.inter), h_last=a(MAX_PREFILL_SEQS, H),
+                        gate_up=a(2, T, cfg.inter) if T > PREFILL_GROUPED_MAX_ROWS else None,
+                        argmax_scratch=torch.zeros(16 * MAX_PREFILL_SEQS + 16, dtype=torch.uint8, device=dev),
+                        q8_scratch=torch.empty(MMVQ_MAX_BATCH * (-(-H // 512) * 16) * 36, dtype=torch.uint8, device=dev))
+        # first tokens [256], then a copy of the runner's context lengths: one D2H copy returns both
+        self._out = torch.zeros(MAX_PREFILL_SEQS + (runner.B if runner is not None else 0), dtype=torch.int32, device=dev)
+        self._layers, self.step_struct = _model_step(weights, self.k_cache, self.v_cache, pdl, cfg.n_heads, cfg.n_kv_heads)
+        self.num_cache_blocks = self.k_cache[0].shape[0]
 
     def forward(self, tokens, all_logits=False, cached=0, table=None):
         """tokens: list[int] (1 < len <= max_tokens), the prompt at positions cached .. cached + T - 1.  Returns logits
@@ -719,68 +752,172 @@ class LlamaPrefill:
         chunks of a chunked prompt); only `tokens` are computed, and they attend to all cached + T keys through the
         paged prefill kernel.  Then T == 1 is allowed.  table: block ids of the sequence (e.g.
         `KVCacheManager.get_block_ids`), default the prefill's own table or the runner's."""
-        from . import mmq, ops, paged_attn, quant
-        cfg, dev, dt, w = self.cfg, self.dev, self.dt, self.w
+        cfg = self.cfg
         T, cached = len(tokens), int(cached)
         bs = cfg.block_size
         if cached == 0 and table is None:
             if not 1 < T <= min(self.max_tokens, cfg.max_pos):
                 raise ValueError(f"LlamaPrefill.forward: need 1 < tokens <= {min(self.max_tokens, cfg.max_pos)}, got {T}")
-            slots = self._slots[:T]
         else:
-            table = self.table if table is None else [int(b) for b in table]
             end = cached + T
+            tb = self.table if table is None else table
             if cached < 0 or not (1 if cached else 2) <= T <= self.max_tokens:
                 raise ValueError(f"LlamaPrefill.forward: need cached >= 0 and {1 if cached else 2} <= tokens <= "
                                  f"{self.max_tokens}, got cached={cached}, {T} tokens")
-            if end > min(cfg.max_pos, len(table) * bs):
+            if end > min(cfg.max_pos, len(tb) * bs):
                 raise ValueError(f"LlamaPrefill.forward: cached + tokens = {end} exceeds max_pos {cfg.max_pos} or the "
-                                 f"table's {len(table)} blocks of {bs}")
-            slots = torch.tensor([table[i // bs] * bs + i % bs for i in range(cached, end)], dtype=torch.int64, device=dev)
-            if cached:
-                positions = torch.arange(cached, end, dtype=torch.int32, device=dev)
-                block_table = torch.tensor([table], dtype=torch.int32, device=dev)
-                cu_q = torch.tensor([0, T], dtype=torch.int32, device=dev)
-                cu_k = torch.tensor([0, end], dtype=torch.int32, device=dev)
-        H, KVH, D = cfg.n_heads, cfg.n_kv_heads, cfg.head_dim
-        if torch.is_tensor(tokens):      # e.g. pinned host ids: the H2D copy is part of the call
-            ids = tokens.to(device=dev, dtype=torch.int32, non_blocking=True)
-        else:
-            ids = torch.tensor(tokens, dtype=torch.int32, device=dev)
-        x = torch.empty(T, cfg.hidden, dtype=dt, device=dev)
-        t, ty, rows, cols = w.tok_embd
-        rc = lib().mrs_embedding_gather(ctypes.c_int32(GGML[ty]), ctypes.c_void_p(t.data_ptr()), ctypes.c_int32(cols),
-                                        ctypes.c_void_p(ids.data_ptr()), ctypes.c_int32(T), ctypes.c_void_p(x.data_ptr()),
-                                        ctypes.c_int32({torch.float16: 0, torch.bfloat16: 1}[dt]),
-                                        ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise RuntimeError(f"mrs_embedding_gather failed with cudaError {rc}")
-        qt = lambda e: quant.QTensor(e[0], e[1], (e[2], e[3]))
-        scale = 1.0 / float(np.sqrt(D))
-        h = ops.rms_norm(x, w.layers[0]["attn_norm"], cfg.rms_eps)
-        for l, L in enumerate(w.layers):
-            q = mmq.forward(qt(L["attn_q"]), h).view(T, H, D)
-            k = mmq.forward(qt(L["attn_k"]), h).view(T, KVH, D)
-            v = mmq.forward(qt(L["attn_v"]), h).view(T, KVH, D)
-            if cached:   # the suffix's K/V go into the cache first, then attend over the whole sequence there
-                ops.apply_rotary_qk(q, k, w.rope_cos, w.rope_sin, positions, is_neox=cfg.rope_neox)
-                paged_attn.reshape_and_cache_flashinfer(k, v, self.k_cache[l], self.v_cache[l], slots)
-                attn = paged_attn.prefill_attention_paged(q, self.k_cache[l], self.v_cache[l], block_table, cu_q, cu_k,
-                                                          T, end, scale)
+                                 f"table's {len(tb)} blocks of {bs}")
+        table = self.table if table is None else [int(b) for b in table]
+        logits = self._step([tokens], [cached], [table], lm_rows=2 if all_logits else 1)
+        return logits if all_logits else logits[0]
+
+    def check_batch_args(self, prompts, cached=None, tables=None, slots=None, final=True):
+        """ValueError for a forward_batch call the step cannot take; returns (token id arrays, cached, tables).  Uses only
+        cfg, max_tokens, table and (optional) runner."""
+        cfg, bs = self.cfg, self.cfg.block_size
+        runner = getattr(self, "runner", None)
+        n = len(prompts)
+        if not 1 <= n <= MAX_PREFILL_SEQS:
+            raise ValueError(f"LlamaPrefill.forward_batch: need 1..{MAX_PREFILL_SEQS} sequences, got {n}")
+        ids = []
+        for p in prompts:
+            a = p.cpu().numpy() if torch.is_tensor(p) else np.asarray(p)
+            a = a.reshape(-1)
+            if a.size and (a.dtype.kind not in "iu" or int(a.min()) < 0 or int(a.max()) >= cfg.vocab):
+                raise ValueError(f"LlamaPrefill.forward_batch: token ids must be integers in [0, {cfg.vocab})")
+            ids.append(a.astype(np.int32))
+        cached = [0] * n if cached is None else [int(c) for c in cached]
+        if len(cached) != n:
+            raise ValueError(f"LlamaPrefill.forward_batch: {len(cached)} cached lengths for {n} sequences")
+        if slots is not None:
+            if not final:
+                raise ValueError("LlamaPrefill.forward_batch: slots commit first tokens, which a non-final chunk has none of")
+            if runner is None:
+                raise ValueError("LlamaPrefill.forward_batch: slots need a LlamaPrefill built with a runner")
+            slots = [int(s) for s in slots]
+            if len(slots) != n:
+                raise ValueError(f"LlamaPrefill.forward_batch: {len(slots)} slots for {n} sequences")
+            if len(set(slots)) != n or min(slots) < 0 or max(slots) >= runner.B:
+                raise ValueError(f"LlamaPrefill.forward_batch: slots must be distinct runner rows in 0..{runner.B - 1}")
+        if tables is None:
+            if slots is not None:
+                tables = [list(runner.tables[s]) for s in slots]
+            elif n == 1:
+                tables = [self.table]
+            elif runner is not None and n <= runner.B:
+                tables = [list(runner.tables[i]) for i in range(n)]
             else:
-                ops.apply_rotary_qk(q, k, w.rope_cos, w.rope_sin, None, is_neox=cfg.rope_neox)
-                attn = paged_attn.prefill_attention(q, k, v, scale)
-                paged_attn.reshape_and_cache_flashinfer(k, v, self.k_cache[l], self.v_cache[l], slots)
-            o = mmq.forward(qt(L["attn_output"]), attn.view(T, H * D))
-            x, h2 = ops.add_rms_norm(o, x, L["ffn_norm"], cfg.rms_eps)       # x = o + x ; h2 = norm(x)
-            gate = mmq.forward(qt(L["ffn_gate"]), h2)
-            up = mmq.forward(qt(L["ffn_up"]), h2)
-            d = mmq.forward(qt(L["ffn_down"]), ops.fused_glu(gate, up, 0))
-            nxt = w.layers[l + 1]["attn_norm"] if l + 1 < cfg.n_layers else w.output_norm
-            x, h = ops.add_rms_norm(d, x, nxt, cfg.rms_eps)                   # x = d + x ; h = next norm(x)
-        if all_logits:
-            return mmq.forward(qt(w.output), h)
-        return quant.plain(qt(w.output), h[T - 1:T].contiguous())[0]
+                raise ValueError("LlamaPrefill.forward_batch: several sequences need their own tables (tables= or a runner)")
+        tables = [[int(b) for b in t] for t in tables]
+        if len(tables) != n:
+            raise ValueError(f"LlamaPrefill.forward_batch: {len(tables)} tables for {n} sequences")
+        total = sum(a.size for a in ids)
+        if total > self.max_tokens:
+            raise ValueError(f"LlamaPrefill.forward_batch: {total} new rows exceed max_tokens {self.max_tokens}")
+        for i, (a, c, t) in enumerate(zip(ids, cached, tables)):
+            if c < 0 or a.size < (1 if c else 2):
+                raise ValueError(f"LlamaPrefill.forward_batch: sequence {i} needs cached >= 0 and at least "
+                                 f"{1 if c else 2} tokens, got cached={c}, {a.size} tokens")
+            cap = len(t) * bs if slots is None else min(len(t), runner.max_blocks) * bs
+            if c + a.size > min(cfg.max_pos, cap):
+                raise ValueError(f"LlamaPrefill.forward_batch: sequence {i}: cached + tokens = {c + a.size} exceeds max_pos "
+                                 f"{cfg.max_pos} or its table's {len(t)} blocks of {bs}")
+        if n > 1:
+            slot_map = np.concatenate([kv_index.slot_mapping(t, bs, c, c + a.size) for a, c, t in zip(ids, cached, tables)])
+            if np.unique(slot_map).size != slot_map.size:
+                raise ValueError("LlamaPrefill.forward_batch: two sequences' new rows map to the same cache slot")
+        return ids, cached, tables, slots
+
+    def forward_batch(self, prompts, cached=None, tables=None, slots=None, final=True):
+        """n sequences' new rows (prompts: n token lists) in one `mrs_llama_prefill_step`.  cached[i] rows of sequence i
+        are already in the cache under tables[i] (default 0); tables default to the runner's (rows slots[i], or 0..n-1),
+        or the prefill's own table for one sequence.  Returns (last-row logits [n, vocab] on the device, first tokens
+        int32 [n] on the host); with final=False (a non-final chunk group) only the KV caches are written and nothing
+        is returned.
+        slots (needs the runner given at construction): sequence i continues in runner row slots[i].  A given tables[i]
+        becomes that row's block table; the step writes each first token and context length into the row on the
+        device, and runner.steps_taken becomes the longest context of the runner.  Rows not in slots are untouched,
+        so a serving loop can refill a finished row between runner.replay() calls."""
+        ids, cached, tables, slots = self.check_batch_args(prompts, cached, tables, slots, final)
+        if not final:
+            self._step(ids, cached, tables, lm_rows=0)
+            return None
+        logits = self._step(ids, cached, tables, lm_rows=1, slots=slots)
+        n = len(ids)
+        if slots is None:
+            return logits, self._out[:n].cpu()
+        r = self.runner
+        self._out[MAX_PREFILL_SEQS:].copy_(r.context_lens)
+        host = self._out.cpu()
+        r.steps_taken = int(host[MAX_PREFILL_SEQS:].max())
+        return logits, host[:n].clone()
+
+    def _step(self, ids, cached, tables, lm_rows, slots=None):
+        """Build the plan, enqueue the step; returns the logits ([n, vocab] for lm_rows 1, [T, vocab] for 2) or None."""
+        p, logits, _plan = self.make_plan(ids, cached, tables, lm_rows, slots)
+        rc = lib().mrs_llama_prefill_step(ctypes.byref(self.step_struct), ctypes.byref(p),
+                                          ctypes.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream))
+        if rc != 0:
+            raise RuntimeError(f"mrs_llama_prefill_step failed: cudaError {rc}")
+        return logits
+
+    def make_plan(self, ids, cached, tables, lm_rows, slots=None):
+        """The step's `mrs_llama_prefill` for checked arguments: the plan is built on the host and sent in one pinned
+        H2D copy (enqueued on the current stream).  With slots, the runner rows' block tables are written as well.
+        Returns (struct, logits or None, device plan tensor the struct points into)."""
+        cfg, dev, bs = self.cfg, self.dev, self.cfg.block_size
+        ids = [np.asarray(p.cpu().numpy() if torch.is_tensor(p) else p, dtype=np.int32).reshape(-1) for p in ids]
+        n = len(ids)
+        lens = np.array([a.size for a in ids], dtype=np.int64)
+        cached = np.asarray(cached, dtype=np.int64)
+        T = int(lens.sum())
+        cu_q = np.concatenate([[0], np.cumsum(lens)])
+        cu_k = np.concatenate([[0], np.cumsum(lens + cached)])
+        paged = bool(cached.any())
+        slot_map = np.concatenate([kv_index.slot_mapping(t, bs, int(c), int(c + l)) for t, c, l in zip(tables, cached, lens)])
+        runner = self.runner if slots is not None else None
+        # one int32 plan: slot_mapping (i64) | token ids | positions | cu_q | cu_k | last rows | dest rows | block tables
+        stride = max(len(t) for t in tables) if (paged or runner is not None) else 0
+        if runner is not None:
+            stride = runner.max_blocks
+        seg = [2 * T, T, T, n + 1, n + 1, n, n, n * stride]
+        off = np.concatenate([[0], np.cumsum(seg)])
+        host = torch.empty(int(off[-1]), dtype=torch.int32, pin_memory=True)
+        hn = host.numpy()
+        hn[off[0]:off[1]] = slot_map.view(np.int32)
+        hn[off[1]:off[2]] = np.concatenate(ids)
+        hn[off[2]:off[3]] = np.concatenate([np.arange(c, c + l) for c, l in zip(cached, lens)])
+        hn[off[3]:off[4]] = cu_q
+        hn[off[4]:off[5]] = cu_k
+        hn[off[5]:off[6]] = cu_q[1:] - 1
+        hn[off[6]:off[7]] = slots if slots is not None else 0
+        bt = hn[off[7]:off[8]].reshape(n, stride) if stride else None
+        if bt is not None:
+            bt[:] = 0
+            for i, t in enumerate(tables):
+                bt[i, :min(len(t), stride)] = t[:stride]
+        plan = host.to(dev, non_blocking=True)
+        ptr = lambda k: plan.data_ptr() + 4 * int(off[k])
+        if runner is not None and bt is not None:   # the rows' block tables, for the decode steps that follow
+            rows = plan[off[6]:off[7]].long()
+            runner.block_tables.index_copy_(0, rows, plan[off[7]:off[8]].view(n, stride))
+            for s, t in zip(slots, tables):
+                runner.tables[s] = list(t)
+        p = _Prefill()
+        p.n_seqs, p.total_tokens, p.max_q_len, p.max_kv_len = n, T, int(lens.max()), int((lens + cached).max())
+        p.paged, p.lm_rows, p.block_table_stride, p.num_blocks = int(paged), int(lm_rows), stride, self.num_cache_blocks
+        p.slot_mapping, p.token_ids, p.positions, p.cu_seqlens_q, p.cu_seqlens_k, p.last_rows = (ptr(k) for k in range(6))
+        p.block_tables = ptr(7) if paged else None
+        for name, t in self.buf.items():
+            setattr(p, name, None if t is None else t.data_ptr())
+        logits = None
+        if lm_rows:
+            logits = torch.empty(n if lm_rows == 1 else T, cfg.vocab, dtype=self.dt, device=dev)
+            p.logits, p.out_token = logits.data_ptr(), self._out.data_ptr()
+        if runner is not None:
+            p.dest_rows = ptr(6)
+            p.runner_token_ids, p.runner_context_lens = runner.meta["token_ids"].data_ptr(), runner.context_lens.data_ptr()
+        return p, logits, plan
 
 
 def check_drafts(drafts, batch, draft_len, vocab):
