@@ -6,8 +6,8 @@
  * enqueues the per-token kernel chain on the given stream (CUDA-graph capturable: no
  * allocation, no host sync).  Per decoder layer it issues
  *     [RMSNorm + Q8_1 + fused QKV GEMV] -> RoPE -> KV-cache write -> paged decode attention
- *     -> [Q8_1 + o_proj GEMV + residual] -> [RMSNorm + Q8_1 + gate/up GEMV + SiLU*mul]
- *     -> [Q8_1 + down GEMV + residual]
+ *     -> [Q8_1 + o_proj GEMV + residual] -> [RMSNorm + Q8_1 + gate/up GEMV + SiLU*mul + Q8_1]
+ *     -> [down GEMV + residual]
  * with the bracketed groups being single `mrs_mmvq_fused` launches.
  */
 #ifndef MRS_B200_MODEL_H
@@ -68,7 +68,8 @@ typedef struct {
   int32_t *request_indices, *kv_tile_indices, *o_indptr, *kv_chunk_size;
   uint8_t *block_valid_mask;
   /* scratch (activation dtype unless noted) */
-  void *x, *x2, *q, *k, *v, *attn_out, *act, *logits; /* x, x2: [batch, hidden] residual stream ping-pong */
+  void *x, *x2, *q, *k, *v, *attn_out, *act, *logits; /* x, x2: [batch, hidden] residual stream ping-pong; on the
+                              * GEMV route (batch <= 8) act holds the block_q8_1 form of the GLU output (36 B per 32) */
   void *tmp_v; float *tmp_s;
   int32_t *out_token;        /* [batch] argmax of the logits */
   int32_t *attn_counters;    /* zeroed int32 [batch * n_kv_heads * 2] (fused attention merge) */

@@ -57,6 +57,10 @@ int mrs_mmvq_has_wide(void);
  * launch_mmvq_gguf_quantize_q8_1_* + launch_mmvq_gguf_*  (+ the residual add).
  * mode 0 plain (w0), 1 fused GLU (w0 = gate, w1 = up), 2 fused QKV (w0,w1[,w2]; n2 may be 0).
  * x [b_size, K] of dtype dt (0 f16 / 1 bf16 / 2 f32), 16-byte aligned; norm_w / residual may be NULL.
+ * mode | 4: x is already block_q8_1 [b_size][K / 32] (norm_w must be NULL) — what a mode | 8 launch wrote.
+ * mode | 8 (fused GLU, n0 % 32 == 0): dst0 receives the block_q8_1 [b_size][n0 / 32] form of the output, byte for
+ * byte what launch_mmvq_gguf_quantize_q8_1_* makes of the dt output; each CTA owns whole 32-row groups.
+ * Results with mode | 4 equal those with the same activations raw, bit for bit.
  * ggml_type: GgmlDType code (2 q4_0 .. 14 q6_k).  Returns a cudaError_t. */
 int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, const void *w1, const void *w2, const void *x,
                    const void *norm_w, float eps, const void *residual, void *dst0, void *dst1, void *dst2, int K,

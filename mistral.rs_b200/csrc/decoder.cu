@@ -536,12 +536,8 @@ static int32_t llama_forward(const mrs_llama_step *s, int q_len, void *stream) {
       MRS_TRY(mrs_mmvq_fused(L.wq.ggml_type, 2, dt, L.wq.data, L.wk.data, L.wv.data, hidden, L.attn_norm, s->rms_eps,
                              nullptr, s->q, s->k, s->v, H, nq, nkv, nkv, B, 0, pdl, stream));
     } else {
-      // Q4_K_M keeps attn_v in Q6_K on some layers: q∥k fused, v on its own.  (Under PDL the small v launch
-      // hides behind the q∥k tail; the one-grid form, mrs_mmvq_fused_qkv_mixed, would take CTAs from q∥k.)
-      MRS_TRY(mrs_mmvq_fused(L.wq.ggml_type, 2, dt, L.wq.data, L.wk.data, nullptr, hidden, L.attn_norm, s->rms_eps,
-                             nullptr, s->q, s->k, nullptr, H, nq, nkv, 0, B, 0, pdl, stream));
-      MRS_TRY(mrs_mmvq_fused(L.wv.ggml_type, 0, dt, L.wv.data, nullptr, nullptr, hidden, L.attn_norm, s->rms_eps,
-                             nullptr, s->v, nullptr, nullptr, H, nkv, 0, 0, B, 0, pdl, stream));
+      MRS_TRY(mrs_mmvq_fused_qkv_mixed(L.wq.ggml_type, L.wv.ggml_type, dt, L.wq.data, L.wk.data, L.wv.data, hidden,
+                                       L.attn_norm, s->rms_eps, s->q, s->k, s->v, H, nq, nkv, nkv, B, pdl, stream));
     }
     if (do_attn && q_len > 1) {
       MRS_TRY(mrs_paged_decode_fused_multi(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
@@ -590,19 +586,22 @@ static int32_t llama_forward(const mrs_llama_step *s, int q_len, void *stream) {
     }
     // --- MLP block: x = x + down(silu(gate(norm(x))) * up(norm(x)))
     if (L.w_gate.ggml_type != L.w_up.ggml_type || L.w_gate.rows != L.w_up.rows) return (int32_t)cudaErrorInvalidValue;
-    MRS_TRY(mrs_mmvq_fused(L.w_gate.ggml_type, 1, dt, L.w_gate.data, L.w_up.data, nullptr, hidden2, L.ffn_norm,
+    // the GLU epilogue writes act in its Q8_1 form (block_q8_1 [B][rows / 32], inside act's B x rows activation-dtype
+    // bytes), the form down_proj consumes: quantised once, not again by every CTA of down_proj
+    const int q8 = (L.w_gate.rows % 32 == 0) ? 1 : 0;
+    MRS_TRY(mrs_mmvq_fused(L.w_gate.ggml_type, 1 | (q8 ? 8 : 0), dt, L.w_gate.data, L.w_up.data, nullptr, hidden2, L.ffn_norm,
                            s->rms_eps, nullptr, s->act, nullptr, nullptr, H, L.w_gate.rows, L.w_gate.rows, 0, B, 0,
                            pdl, stream));
     if (s->tp != nullptr && s->tp->world > 1) {
       void *part = (uint8_t *)s->tp->peer_base[s->tp->rank] + s->tp->slot_offset[1];
-      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, nullptr,
+      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, q8 ? 4 : 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, nullptr,
                              part, nullptr, nullptr, L.w_down.cols, H, 0, 0, B, 0, pdl, stream));
       MRS_TRY(mrs_tp_allreduce_residual(s->tp, 1, hidden2, hidden, B * H, dt, pdl, stream));
     } else if (s->all_reduce == nullptr) {
-      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, hidden2,
+      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, q8 ? 4 : 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, hidden2,
                              hidden, nullptr, nullptr, L.w_down.cols, H, 0, 0, B, 0, pdl, stream));
     } else {
-      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, nullptr,
+      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, q8 ? 4 : 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, nullptr,
                              hidden, nullptr, nullptr, L.w_down.cols, H, 0, 0, B, 0, pdl, stream));
       s->all_reduce(hidden, (int64_t)B * H, dt, stream, s->all_reduce_user);
       add_residual_kernel<<<(unsigned)(((int64_t)B * H + 255) / 256), 256, 0, st>>>(hidden, hidden2, (int64_t)B * H, dt);

@@ -62,6 +62,7 @@ struct MmvqParams {
   int K, stride_col_y, stride_col_dst, ncols;
   int mode, activation, dst_dtype;
   int nstages, vrows, pdl, flags;
+  int dst_q8;            // MODE_GLU: dst[0] is block_q8_1[ncols][stride_col_dst], the Q8_1 form of the output
 #ifdef MRS_TIMELINE
   unsigned long long *dbg;  // dev build: [gridDim.x][16] globaltimer stamps of this launch
 #endif
@@ -175,10 +176,12 @@ __device__ __forceinline__ void mmvq_body(const MmvqParams &p, const int cta, co
   const uint32_t off_xq0 = 256;
   const uint32_t off_xq1 = off_xq0 + (uint32_t)NCOLS * npos * 16;
   const uint32_t off_xa = off_xq1 + (uint32_t)NCOLS * npos * 16;
-  const uint32_t off_ring = (off_xa + (uint32_t)NCOLS * npos * Q::AUX * 4 + 127u) & ~127u;
+  const uint32_t off_qb = off_xa + (uint32_t)NCOLS * npos * Q::AUX * 4;
+  const uint32_t off_ring = (off_qb + (p.dst_q8 ? 2u * NCOLS * 32 * 4 : 0u) + 127u) & ~127u;
   int4 *xq0 = (int4 *)(smem + off_xq0);   // [NCOLS][npos]
   int4 *xq1 = (int4 *)(smem + off_xq1);   // [NCOLS][npos]
   float *xa = (float *)(smem + off_xa);   // [NCOLS][npos][AUX]
+  float *qb = (float *)(smem + off_qb);   // dst_q8: [2][NCOLS][32] GLU outputs of a 32-row group, double-buffered
   uint8_t *ring = smem + off_ring;
 
   if (tid == 0) {
@@ -189,9 +192,10 @@ __device__ __forceinline__ void mmvq_body(const MmvqParams &p, const int cta, co
   __syncthreads();
   if (tid == 0) MRS_STAMP(1);
 
-  // contiguous virtual-row range of this CTA
-  const int vr0 = (int)((long long)p.vrows * cta / ncta);
-  const int vr1 = (int)((long long)p.vrows * (cta + 1) / ncta);
+  // contiguous virtual-row range of this CTA; a launch that writes Q8_1 hands out whole 32-row groups (one block each)
+  const int gran = p.dst_q8 ? 32 : 1;
+  const int vr0 = gran * (int)((long long)(p.vrows / gran) * cta / ncta);
+  const int vr1 = gran * (int)((long long)(p.vrows / gran) * (cta + 1) / ncta);
   const int P = (p.mode == MODE_GLU) ? NCW : SLOTS;  // virtual rows per pass
 
   if (warp == NCW) {
@@ -255,7 +259,9 @@ __device__ __forceinline__ void mmvq_body(const MmvqParams &p, const int cta, co
   if (p.pdl) pdl_wait();  // activations come from the upstream kernel
   if (tid == 0) MRS_STAMP(3);
   if (p.xkind == X_Q8_1) {
-    // gather pre-quantised Q8_1 blocks straight into consumption order
+    // gather pre-quantised Q8_1 blocks straight into consumption order.  QT::aux over the blocks yields the same floats
+    // as QT::chunk_aux in the raw prologue below (same half-rounded d / sum, same integer sums), so a launch fed Q8_1
+    // computes bit for bit what it computes from the raw activations (tests/test_mmvq_q8_io_gpu.py)
     const block_q8_1 *y = (const block_q8_1 *)p.x;
     for (int idx = ctid; idx < NCOLS * npos; idx += NCT) {
       const int col = idx / npos, pos = idx - col * npos;
@@ -490,7 +496,8 @@ __device__ __forceinline__ void mmvq_body(const MmvqParams &p, const int cta, co
               const float g = round_act(acc[0][j], p.dst_dtype);
               const float up = round_act(acc[1][j], p.dst_dtype);
               const float act = round_act(glu_activation(g, p.activation), p.dst_dtype);
-              store_act(p.dst[0], (int64_t)j * p.stride_col_dst + rr[0], act * up, p.dst_dtype);
+              if (p.dst_q8) qb[(((base - vr0) >> 5) & 1) * NCOLS * 32 + j * 32 + ((base - vr0) & 31) + warp] = round_act(act * up, p.dst_dtype);
+              else store_act(p.dst[0], (int64_t)j * p.stride_col_dst + rr[0], act * up, p.dst_dtype);
             }
           }
         }
@@ -510,6 +517,27 @@ __device__ __forceinline__ void mmvq_body(const MmvqParams &p, const int cta, co
               }
               store_act(p.dst[mm[r]], (int64_t)j * cs + rr[r], v, p.dst_dtype);
             }
+          }
+        }
+      }
+    }
+    if (p.dst_q8 && ((base + P - vr0) & 31) == 0) {
+      // the 32 rows of this group are in qb: warp 0 writes their block_q8_1 with the arithmetic of the standalone
+      // quantiser (quantize_q8_1_kernel: lane = element, warp_max / warp_sum, fast divisions, half d and sum)
+      asm volatile("bar.sync 1, %0;" ::"n"(NCT));
+      if (warp == 0) {
+        const float *src = qb + (((base - vr0) >> 5) & 1) * NCOLS * 32;
+        const int blk = (base + P - 32) >> 5;
+#pragma unroll
+        for (int j = 0; j < NCOLS; j++) {
+          if (j < p.ncols) {
+            const float v = src[j * 32 + lane];
+            const float amax = warp_max(fabsf(v));
+            const float sum = warp_sum(v);
+            const float d = __fdividef(amax, 127.0f);
+            block_q8_1 *yb = (block_q8_1 *)p.dst[0] + (size_t)j * p.stride_col_dst + blk;
+            yb->qs[lane] = (amax == 0.0f) ? (int8_t)0 : (int8_t)roundf(__fdividef(v, d));
+            if (lane == 0) yb->ds = __halves2half2(__float2half_rn(d), __float2half_rn(sum));
           }
         }
       }
@@ -579,7 +607,7 @@ static bool plan8(const MmvqParams &p, int ncols, const DevInfo &d, int &nst, si
   const int nblocks = p.K / QT<T>::QK;
   const int nseg = (nblocks + G::SEG_BLOCKS - 1) / G::SEG_BLOCKS;
   const int npos = nseg * G::SEG_UNITS;
-  const size_t xbytes = 256 + (size_t)ncols * npos * G::XU_BYTES + 128;
+  const size_t xbytes = 256 + (size_t)ncols * npos * G::XU_BYTES + (p.dst_q8 ? 2 * (size_t)ncols * 32 * 4 : 0) + 128;
   // batch 1 may run three CTAs per SM (72-register kernels): 24 consumer warps hide the shared-memory
   // and dp4a latencies better than 16
   ctas_per_sm = (ncols == 1) ? g_ctas_per_sm : (g_ctas_per_sm > 2 ? 2 : g_ctas_per_sm);
@@ -617,6 +645,7 @@ static cudaError_t launch_one(MmvqParams p, cudaStream_t stream) {
 #endif
   const int P = (p.mode == MODE_GLU) ? NCW : SLOTS;
   int grid = (p.vrows + P - 1) / P;
+  if (p.dst_q8) grid = p.vrows / 32;  // whole 32-row groups per CTA
   const int max_grid = ctas_per_sm * d.num_sms;
   if (grid > max_grid) grid = max_grid;
   if (grid < 1) grid = 1;
@@ -861,18 +890,26 @@ MRS_MMVQ_TYPE(q6_k, MRS_Q6_K)
 static cudaError_t mmvq_dispatch_dual_entry(int t1, const MmvqParams &pa, int t2, const MmvqParams &pb, cudaStream_t stream);
 
 // ---- native fused entry points (same arithmetic, fewer launches) ------------------------
-// y = W . q8_1( [rmsnorm_w *] x ) [+ residual]; mode 0 plain, 1 fused GLU, 2 fused QKV.
+// y = W . q8_1( [rmsnorm_w *] x ) [+ residual]; mode bits 0-1: 0 plain, 1 fused GLU, 2 fused QKV.
 // x is raw activations [b_size, K] of dtype `dt`; norm_w may be NULL; residual may be NULL.
+// mode bit 2 (4): x is already block_q8_1 [b_size][K / 32] (norm_w must be NULL).
+// mode bit 3 (8, fused GLU only, n0 % 32 == 0): dst0 receives the block_q8_1 [b_size][n0 / 32] form of the
+// output instead of the output, bit for bit what launch_mmvq_gguf_quantize_q8_1_* makes of it.
 extern "C" int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, const void *w1, const void *w2,
                               const void *x, const void *norm_w, float eps, const void *residual,
                               void *dst0, void *dst1, void *dst2, int K, int n0, int n1, int n2,
                               int b_size, int activation, int pdl, void *stream) {
+  const bool xq8 = (mode & 4) != 0, yq8 = (mode & 8) != 0;
+  if (mode & ~15) return (int)cudaErrorInvalidValue;
+  mode &= 3;
+  if (mode == 3 || (xq8 && norm_w != nullptr) || (yq8 && (mode != MODE_GLU || n0 % 32 != 0))) return (int)cudaErrorInvalidValue;
   MmvqParams p = {};
   p.w[0] = (const uint8_t *)w0; p.w[1] = (const uint8_t *)w1; p.w[2] = (const uint8_t *)w2;
   p.dst[0] = dst0; p.dst[1] = dst1; p.dst[2] = dst2;
   p.nrows[0] = n0; p.nrows[1] = n1; p.nrows[2] = n2;
-  p.x = x; p.xkind = X_RAW; p.xdtype = dt; p.norm_w = norm_w; p.eps = eps; p.residual = residual;
-  p.K = K; p.stride_col_dst = n0; p.ncols = b_size; p.mode = mode; p.activation = activation;
+  p.x = x; p.xkind = xq8 ? X_Q8_1 : X_RAW; p.stride_col_y = K / 32; p.xdtype = dt; p.norm_w = norm_w; p.eps = eps;
+  p.residual = residual; p.dst_q8 = yq8;
+  p.K = K; p.stride_col_dst = yq8 ? n0 / 32 : n0; p.ncols = b_size; p.mode = mode; p.activation = activation;
   p.dst_dtype = dt; p.pdl = pdl;
   p.vrows = (mode == MODE_QKV) ? n0 + n1 + n2 : n0;
   return (int)mmvq_dispatch(ggml_type, p, (cudaStream_t)stream);
