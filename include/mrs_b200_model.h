@@ -89,7 +89,10 @@ typedef struct {
  * accumulation, the prefill GEMM's numerics).  Per layer: grouped QKV (one launch, or q|k + v when attn_v has its own
  * type) -> the same attention -> o GEMM -> add + RMSNorm -> gate|up GEMM with the SiLU*mul epilogue -> down GEMM
  * -> add + RMSNorm with the next layer's norm; then the lm_head GEMM and argmax.  Needs `h`; skip_mask bit 1 skips
- * the GEMMs; cudaErrorInvalidValue with tp or all_reduce set (no tensor parallelism above 8 rows). */
+ * the GEMMs.
+ * cudaErrorInvalidValue, before any launch, for: batch outside 1..256; (batch >= 9) tp or all_reduce set (no tensor
+ * parallelism above 8 rows), a NULL h or an activation dtype other than f16 / bf16; a NULL `layers` with n_layers >= 1;
+ * a layer whose w_gate and w_up differ in ggml type or rows. */
 int32_t mrs_llama_decode_step(const mrs_llama_step *s, void *stream);
 
 /* On-device restatement of the scheduler-side index producers for a running decode batch
@@ -131,9 +134,10 @@ int32_t mrs_decode_advance(const int32_t *block_tables, int32_t max_blocks_per_s
  *   B 1..8:   the GEMV chain, B*q_len <= 8 rows;
  *   B 9..256: the wgmma dequant-GEMM chain (prefill GEMM numerics) over B*q_len rows, up to 2048; needs `h` and an
  *             f16 / bf16 activation dtype.
- * Graph-capturable.  skip_mask as for decode.  cudaErrorInvalidValue for B outside 1..256, B <= 8 with B*q_len > 8,
- * q_len outside 2..8, fused_attention == 0, head_dim other than 64 / 128, tp / all_reduce set, out_token ==
- * token_ids, a NULL context_lens / accepted / emitted, or (B >= 9) a NULL h or another activation dtype. */
+ * Graph-capturable.  skip_mask as for decode.  cudaErrorInvalidValue, before any launch, for B outside 1..256, B <= 8
+ * with B*q_len > 8, q_len outside 2..8, fused_attention == 0, head_dim other than 64 / 128, tp / all_reduce set,
+ * out_token == token_ids, a NULL context_lens / accepted / emitted, (B >= 9) a NULL h or another activation dtype, or
+ * the model faults of mrs_llama_decode_step (NULL layers, mismatched w_gate / w_up). */
 int32_t mrs_decode_advance_multi(const int32_t *block_tables, int32_t max_blocks_per_seq, int32_t *context_lens,
                                  int32_t batch, int32_t block_size, int32_t split_pages, int32_t padded_tiles,
                                  int32_t *positions, int64_t *slot_mapping, int32_t *kv_indptr, int32_t *kv_indices,
@@ -205,7 +209,9 @@ typedef struct {
  * x / x2 / h / q / k / v / attn_out / act; gate_up when T > 2048; block_tables, with block_table_stride and num_blocks >= 1, when paged; last_rows, h_last, logits, out_token,
  * argmax_scratch, and q8_scratch for n <= 8, when lm_rows == 1; logits when lm_rows == 2; runner_token_ids and
  * runner_context_lens when dest_rows is set); an activation dtype other than f16 / bf16; tensor parallelism (s->tp or
- * s->all_reduce set); lm_rows outside 0..2; dest_rows set while lm_rows != 1; paged outside 0..1. */
+ * s->all_reduce set); lm_rows outside 0..2; dest_rows set while lm_rows != 1; paged outside 0..1; a NULL s->layers; a
+ * layer whose w_gate and w_up differ in ggml type or rows; (lm_rows == 1, n <= 8) an lm_head type without an MMVQ
+ * launcher. */
 int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_llama_prefill *p, void *stream);
 
 /* rows of a quantised table -> activation dtype (embedding gather). ids on device. */

@@ -9,8 +9,32 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
 #define MRS_WARP 32
+
+// host: return a failing call's error code from the enclosing function, naming the call on stderr
+#define MRS_TRY(expr)                                               \
+  do {                                                              \
+    const int _e = (int)(expr);                                     \
+    if (_e != 0) {                                                  \
+      fprintf(stderr, "mrs_b200: %s -> cudaError %d\n", #expr, _e); \
+      return _e;                                                    \
+    }                                                               \
+  } while (0)
+
+// host: launch `kernel` on `stream`, as a programmatic dependent of the previous launch when `pdl` is set
+template <typename... KArgs, typename... Args>
+static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                                     bool pdl, Args &&...args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kernel, static_cast<Args &&>(args)...);
+}
 
 // ggml dtype codes (candle GgmlDType numbering used by the reference's Rust side)
 enum : int {

@@ -10,7 +10,6 @@
 #include "dequant.cuh"
 #include "mrs_b200_model.h"
 
-#include <stdio.h>
 
 extern "C" int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, const void *w1, const void *w2,
                               const void *x, const void *norm_w, float eps, const void *residual, void *dst0,
@@ -404,13 +403,8 @@ extern "C" int32_t mrs_argmax(const void *logits, int32_t rows, int32_t cols, in
   unsigned int *counts = (unsigned int *)(keys + rows);
   int chunks = (cols + 4095) / 4096;
   if (chunks > 64) chunks = 64;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(chunks, rows); cfg.blockDim = dim3(256); cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  return (int32_t)cudaLaunchKernelEx(&cfg, argmax_kernel, logits, (int)cols, (int)act_dtype, out, keys, counts, (int)pdl);
+  return (int32_t)launch_pdl(argmax_kernel, dim3(chunks, rows), dim3(256), 0, (cudaStream_t)stream, pdl, logits, (int)cols,
+                             (int)act_dtype, out, keys, counts, (int)pdl);
 }
 
 extern "C" int32_t mrs_decode_advance(const int32_t *block_tables, int32_t max_blocks_per_seq, int32_t *context_lens,
@@ -419,13 +413,9 @@ extern "C" int32_t mrs_decode_advance(const int32_t *block_tables, int32_t max_b
                                       int32_t *kv_indices, int32_t *kv_last_page_len, int32_t *request_indices,
                                       int32_t *kv_tile_indices, int32_t *o_indptr, int32_t *kv_chunk_size,
                                       uint8_t *block_valid_mask, int32_t max_pos, int32_t *error_flag, void *stream) {
-  if (batch < 1 || batch > ADV_MAX_BATCH || max_blocks_per_seq < 1 || block_size < 1) return (int32_t)cudaErrorInvalidValue;
-  decode_advance_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(block_tables, max_blocks_per_seq, context_lens, batch,
-                                                             block_size, split_pages, padded_tiles, max_pos, positions,
-                                                             slot_mapping, kv_indptr, kv_indices, kv_last_page_len,
-                                                             request_indices, kv_tile_indices, o_indptr, kv_chunk_size,
-                                                             block_valid_mask, error_flag, 1);
-  return (int32_t)cudaGetLastError();
+  return mrs_decode_advance_multi(block_tables, max_blocks_per_seq, context_lens, batch, block_size, split_pages, padded_tiles,
+                                  positions, slot_mapping, kv_indptr, kv_indices, kv_last_page_len, request_indices,
+                                  kv_tile_indices, o_indptr, kv_chunk_size, block_valid_mask, max_pos, error_flag, 1, stream);
 }
 
 extern "C" int32_t mrs_decode_advance_multi(const int32_t *block_tables, int32_t max_blocks_per_seq, int32_t *context_lens,
@@ -451,14 +441,8 @@ extern "C" int32_t mrs_spec_accept(const int32_t *argmax, int32_t *token_ids, co
                                    int32_t *context_lens, int32_t *accepted, int32_t *emitted, int32_t batch, int32_t q_len,
                                    int32_t pdl, void *stream) {
   if (batch < 1 || q_len < 1) return (int32_t)cudaErrorInvalidValue;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((batch + 127) / 128); cfg.blockDim = dim3(128); cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  return (int32_t)cudaLaunchKernelEx(&cfg, spec_accept_kernel, argmax, token_ids, slot_mapping, context_lens, accepted,
-                                     emitted, (int)batch, (int)q_len, (int)pdl);
+  return (int32_t)launch_pdl(spec_accept_kernel, dim3((batch + 127) / 128), dim3(128), 0, (cudaStream_t)stream, pdl, argmax,
+                             token_ids, slot_mapping, context_lens, accepted, emitted, (int)batch, (int)q_len, (int)pdl);
 }
 
 extern "C" int32_t mrs_tp_allreduce_residual(const mrs_tp_ctx *ctx, int32_t slot, const void *residual, void *out,
@@ -478,44 +462,88 @@ extern "C" int32_t mrs_tp_allreduce_residual(const mrs_tp_ctx *ctx, int32_t slot
     if ((int64_t)count * 4 > ctx->ll_src_stride) return (int32_t)cudaErrorInvalidValue;
     int th = (count / 2 + 31) / 32 * 32;
     if (th > 1024) th = 1024;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(1); cfg.blockDim = dim3(th); cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
     // the partial of this rank: its slot in the symmetric buffer (what the row-parallel GEMV wrote)
     const void *partial = (const uint8_t *)ctx->peer_base[ctx->rank] + ctx->slot_offset[slot];
-    return (int32_t)cudaLaunchKernelEx(&cfg, tp_allreduce_ll_kernel, c, (int)slot, partial, residual, out, (int)count, (int)dtype, (int)pdl);
+    return (int32_t)launch_pdl(tp_allreduce_ll_kernel, dim3(1), dim3(th), 0, (cudaStream_t)stream, pdl, c, (int)slot, partial,
+                               residual, out, (int)count, (int)dtype, (int)pdl);
   }
   int threads = (count / 8 + 31) / 32 * 32;
   if (threads > 1024) threads = 1024;
   if (threads < 32) threads = 32;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(1); cfg.blockDim = dim3(threads); cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  return (int32_t)cudaLaunchKernelEx(&cfg, tp_allreduce_residual_kernel, c, (int)slot, residual, out, (int)count, (int)dtype, (int)pdl);
+  return (int32_t)launch_pdl(tp_allreduce_residual_kernel, dim3(1), dim3(threads), 0, (cudaStream_t)stream, pdl, c, (int)slot,
+                             residual, out, (int)count, (int)dtype, (int)pdl);
 }
 
-#define MRS_TRY(expr)                                  \
-  do {                                                 \
-    const int _e = (int)(expr);                        \
-    if (_e != 0) {                                     \
-      fprintf(stderr, "mrs_b200: %s -> cudaError %d\n", #expr, _e); \
-      return _e;                                       \
-    }                                                  \
-  } while (0)
+// cudaErrorInvalidValue for a model the layer chains cannot run, checked before a step's first launch: a NULL layer
+// array, or a layer whose gate and up differ in ggml type or rows (every route runs them as one gate|up launch)
+static int32_t check_model(const mrs_llama_step *s) {
+  if (s->n_layers >= 1 && s->layers == nullptr) return (int32_t)cudaErrorInvalidValue;
+  for (int l = 0; l < s->n_layers; l++) {
+    const mrs_llama_layer &L = s->layers[l];
+    if (L.w_gate.ggml_type != L.w_up.ggml_type || L.w_gate.rows != L.w_up.rows) return (int32_t)cudaErrorInvalidValue;
+  }
+  return 0;
+}
 
-// the layer stack + lm_head + argmax over batch * q_len token rows; q_len > 1 is a speculative verify step (every
-// sequence's rows attend through mrs_paged_decode_fused_multi), q_len == 1 the decode step
+// the decode attention of layer L over s->batch sequences of q_len rows each: mrs_paged_decode_fused_multi for a verify
+// step (q_len > 1), else mrs_paged_decode_fused, or with fused_attention == 0 the RoPE -> KV scatter -> paged decode chain
+static int32_t decode_attention(const mrs_llama_step *s, const mrs_llama_layer &L, int q_len, void *stream) {
+  const int B = s->batch, dt = s->act_dtype, nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
+  const int flags = s->pdl | (s->rope_neox ? 0 : 2);
+  void *tmp_v = s->padded_tiles > B ? s->tmp_v : nullptr;
+  float *tmp_s = s->padded_tiles > B ? s->tmp_s : nullptr;
+  if (q_len > 1)
+    return mrs_paged_decode_fused_multi(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
+                                        s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
+                                        s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
+                                        s->block_valid_mask, s->attn_out, tmp_v, tmp_s, s->attn_counters, B, s->padded_tiles,
+                                        s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
+                                        flags, q_len, stream);
+  if (s->fused_attention)
+    return mrs_paged_decode_fused(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
+                                  s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len, s->request_indices,
+                                  s->kv_tile_indices, s->o_indptr, s->kv_chunk_size, s->block_valid_mask, s->attn_out, tmp_v,
+                                  tmp_s, s->attn_counters, B, s->padded_tiles, s->n_heads, s->n_kv_heads, s->head_dim,
+                                  s->block_size, s->sm_scale, (uint32_t)dt, flags, stream);
+  rotary_embedding_positions(s->q, s->k, (void *)s->rope_cos, (void *)s->rope_sin, s->positions, s->rope_neox, s->head_dim,
+                             B, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt, (int64_t)stream);
+  reshape_and_cache_flashinfer(s->k, s->v, L.k_cache, L.v_cache, s->slot_mapping, B, s->n_kv_heads, s->head_dim,
+                               s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, (cudaStream_t)stream);
+  return flashinfer_decode(s->q, L.k_cache, L.v_cache, s->kv_indptr, s->kv_indices, s->kv_last_page_len, s->request_indices,
+                           s->kv_tile_indices, s->o_indptr, s->kv_chunk_size, (const bool *)s->block_valid_mask, s->attn_out,
+                           tmp_v, tmp_s, B, s->padded_tiles, s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, nq,
+                           s->head_dim, s->sm_scale, -1, 0.f, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, (cudaStream_t)stream);
+}
+
+// the GEMV chain (batch 1..8): the layer stack + lm_head + argmax over batch * q_len token rows; q_len > 1 is a
+// speculative verify step, q_len == 1 the decode step
 static int32_t llama_forward(const mrs_llama_step *s, int q_len, void *stream) {
-  const int dt = s->act_dtype, NS = s->batch, B = s->batch * q_len, H = s->hidden, pdl = s->pdl;
+  if (const int32_t e = check_model(s)) return e;
+  const int dt = s->act_dtype, B = s->batch * q_len, H = s->hidden, pdl = s->pdl;
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
-  cudaStream_t st = (cudaStream_t)stream;
   const bool do_attn = !(s->skip_mask & 1), do_gemv = !(s->skip_mask & 2);
+  const mrs_tp_ctx *tp = (s->tp != nullptr && s->tp->world > 1) ? s->tp : nullptr;
+  // a row-parallel projection: dst = residual + W x.  Single GPU: the GEMV's residual epilogue.  Tensor parallel: the
+  // partial sums of every rank summed, then the residual added: the peer-memory sum (one kernel on the PDL chain, the
+  // partial in this rank's slot buffer), or the all_reduce callback and add_residual_kernel (REF
+  // distributed/layers.rs:965-975)
+  auto row_parallel = [&](const mrs_qweight &W, int mode, const void *x, int K, const void *residual, void *dst,
+                          int slot) -> int32_t {
+    if (tp != nullptr) {
+      void *part = (uint8_t *)tp->peer_base[tp->rank] + tp->slot_offset[slot];
+      MRS_TRY(mrs_mmvq_fused(W.ggml_type, mode, dt, W.data, nullptr, nullptr, x, nullptr, 0.f, nullptr, part, nullptr,
+                             nullptr, K, H, 0, 0, B, 0, pdl, stream));
+      return mrs_tp_allreduce_residual(tp, slot, residual, dst, B * H, dt, pdl, stream);
+    }
+    MRS_TRY(mrs_mmvq_fused(W.ggml_type, mode, dt, W.data, nullptr, nullptr, x, nullptr, 0.f,
+                           s->all_reduce == nullptr ? residual : nullptr, dst, nullptr, nullptr, K, H, 0, 0, B, 0, pdl, stream));
+    if (s->all_reduce != nullptr) {
+      s->all_reduce(dst, (int64_t)B * H, dt, stream, s->all_reduce_user);
+      add_residual_kernel<<<(unsigned)(((int64_t)B * H + 255) / 256), 256, 0, (cudaStream_t)stream>>>(dst, residual,
+                                                                                                    (int64_t)B * H, dt);
+    }
+    return 0;
+  };
 
   MRS_TRY(mrs_embedding_gather(s->tok_embd.ggml_type, s->tok_embd.data, H, s->token_ids, B, s->x, dt, stream));
   void *hidden = s->x, *hidden2 = s->x2;
@@ -539,184 +567,139 @@ static int32_t llama_forward(const mrs_llama_step *s, int q_len, void *stream) {
       MRS_TRY(mrs_mmvq_fused_qkv_mixed(L.wq.ggml_type, L.wv.ggml_type, dt, L.wq.data, L.wk.data, L.wv.data, hidden,
                                        L.attn_norm, s->rms_eps, s->q, s->k, s->v, H, nq, nkv, nkv, B, pdl, stream));
     }
-    if (do_attn && q_len > 1) {
-      MRS_TRY(mrs_paged_decode_fused_multi(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
-                                           s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
-                                           s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                                           s->block_valid_mask, s->attn_out, s->padded_tiles > NS ? s->tmp_v : nullptr,
-                                           s->padded_tiles > NS ? s->tmp_s : nullptr, s->attn_counters, NS, s->padded_tiles,
-                                           s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
-                                           pdl | (s->rope_neox ? 0 : 2), q_len, stream));
-    } else if (do_attn && s->fused_attention) {
-      MRS_TRY(mrs_paged_decode_fused(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
-                                     s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
-                                     s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                                     s->block_valid_mask, s->attn_out, s->padded_tiles > B ? s->tmp_v : nullptr,
-                                     s->padded_tiles > B ? s->tmp_s : nullptr, s->attn_counters, B, s->padded_tiles,
-                                     s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
-                                     pdl | (s->rope_neox ? 0 : 2), stream));
-    } else if (do_attn) {
-    rotary_embedding_positions(s->q, s->k, (void *)s->rope_cos, (void *)s->rope_sin, s->positions, s->rope_neox,
-                               s->head_dim, B, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt,
-                               (int64_t)stream);
-    reshape_and_cache_flashinfer(s->k, s->v, L.k_cache, L.v_cache, s->slot_mapping, B, s->n_kv_heads, s->head_dim,
-                                 s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
-    MRS_TRY(flashinfer_decode(s->q, L.k_cache, L.v_cache, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
-                              s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                              (const bool *)s->block_valid_mask, s->attn_out, s->padded_tiles > B ? s->tmp_v : nullptr,
-                              s->padded_tiles > B ? s->tmp_s : nullptr, B, s->padded_tiles, s->n_heads, s->n_kv_heads,
-                              s->head_dim, s->block_size, nq, s->head_dim, s->sm_scale, -1, 0.f, 1.f, 1.f,
-                              (uint32_t)dt, (uint32_t)dt, st));
-    }
+    if (do_attn) MRS_TRY(decode_attention(s, L, q_len, stream));
     if (!do_gemv) continue;
-    if (s->tp != nullptr && s->tp->world > 1) {
-      // row-parallel partial -> this rank's slot buffer -> peer-memory sum + residual (one kernel, on the PDL chain)
-      void *part = (uint8_t *)s->tp->peer_base[s->tp->rank] + s->tp->slot_offset[0];
-      MRS_TRY(mrs_mmvq_fused(L.wo.ggml_type, 0, dt, L.wo.data, nullptr, nullptr, s->attn_out, nullptr, 0.f, nullptr,
-                             part, nullptr, nullptr, nq, H, 0, 0, B, 0, pdl, stream));
-      MRS_TRY(mrs_tp_allreduce_residual(s->tp, 0, hidden, hidden2, B * H, dt, pdl, stream));
-    } else if (s->all_reduce == nullptr) {
-      MRS_TRY(mrs_mmvq_fused(L.wo.ggml_type, 0, dt, L.wo.data, nullptr, nullptr, s->attn_out, nullptr, 0.f, hidden,
-                             hidden2, nullptr, nullptr, nq, H, 0, 0, B, 0, pdl, stream));
-    } else {  // row-parallel: partial sums -> all-reduce -> residual add (REF distributed/layers.rs:965-975)
-      MRS_TRY(mrs_mmvq_fused(L.wo.ggml_type, 0, dt, L.wo.data, nullptr, nullptr, s->attn_out, nullptr, 0.f, nullptr,
-                             hidden2, nullptr, nullptr, nq, H, 0, 0, B, 0, pdl, stream));
-      s->all_reduce(hidden2, (int64_t)B * H, dt, stream, s->all_reduce_user);
-      add_residual_kernel<<<(unsigned)(((int64_t)B * H + 255) / 256), 256, 0, st>>>(hidden2, hidden, (int64_t)B * H, dt);
-    }
+    MRS_TRY(row_parallel(L.wo, 0, s->attn_out, nq, hidden, hidden2, 0));
     // --- MLP block: x = x + down(silu(gate(norm(x))) * up(norm(x)))
-    if (L.w_gate.ggml_type != L.w_up.ggml_type || L.w_gate.rows != L.w_up.rows) return (int32_t)cudaErrorInvalidValue;
     // the GLU epilogue writes act in its Q8_1 form (block_q8_1 [B][rows / 32], inside act's B x rows activation-dtype
     // bytes), the form down_proj consumes: quantised once, not again by every CTA of down_proj
     const int q8 = (L.w_gate.rows % 32 == 0) ? 1 : 0;
     MRS_TRY(mrs_mmvq_fused(L.w_gate.ggml_type, 1 | (q8 ? 8 : 0), dt, L.w_gate.data, L.w_up.data, nullptr, hidden2, L.ffn_norm,
                            s->rms_eps, nullptr, s->act, nullptr, nullptr, H, L.w_gate.rows, L.w_gate.rows, 0, B, 0,
                            pdl, stream));
-    if (s->tp != nullptr && s->tp->world > 1) {
-      void *part = (uint8_t *)s->tp->peer_base[s->tp->rank] + s->tp->slot_offset[1];
-      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, q8 ? 4 : 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, nullptr,
-                             part, nullptr, nullptr, L.w_down.cols, H, 0, 0, B, 0, pdl, stream));
-      MRS_TRY(mrs_tp_allreduce_residual(s->tp, 1, hidden2, hidden, B * H, dt, pdl, stream));
-    } else if (s->all_reduce == nullptr) {
-      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, q8 ? 4 : 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, hidden2,
-                             hidden, nullptr, nullptr, L.w_down.cols, H, 0, 0, B, 0, pdl, stream));
-    } else {
-      MRS_TRY(mrs_mmvq_fused(L.w_down.ggml_type, q8 ? 4 : 0, dt, L.w_down.data, nullptr, nullptr, s->act, nullptr, 0.f, nullptr,
-                             hidden, nullptr, nullptr, L.w_down.cols, H, 0, 0, B, 0, pdl, stream));
-      s->all_reduce(hidden, (int64_t)B * H, dt, stream, s->all_reduce_user);
-      add_residual_kernel<<<(unsigned)(((int64_t)B * H + 255) / 256), 256, 0, st>>>(hidden, hidden2, (int64_t)B * H, dt);
-    }
+    MRS_TRY(row_parallel(L.w_down, q8 ? 4 : 0, s->act, L.w_down.cols, hidden2, hidden, 1));
   }
   if (do_gemv)
   MRS_TRY(mrs_mmvq_fused(s->lm_head.ggml_type, 0, dt, s->lm_head.data, nullptr, nullptr, hidden, s->final_norm,
                          s->rms_eps, nullptr, s->logits, nullptr, nullptr, H, s->vocab, 0, 0, B, 0, pdl, stream));
   MRS_TRY(mrs_argmax(s->logits, B, s->vocab, dt, s->out_token, s->argmax_scratch, pdl, stream));
-  return 0;
+  return (int32_t)cudaGetLastError();
 }
 
-// the decode step for 9..256 sequences: the reference's GgmlMatMul sends batches above 8 rows to MMQ, so the linears are
-// the wgmma dequant GEMM (mrs_mmq_gguf_grouped) with the prefill GEMM's numerics.  The norms are their own launches
-// (the GEMM reads X through the TMA, unmodified), into the normed-activation buffer s->h.  Per layer:
-//   grouped QKV -> attention (as the GEMV route) -> o GEMM (into h) -> add + RMSNorm (x2 = o + x, h = norm)
-//   -> gate|up GEMM with the GLU epilogue (act) -> down GEMM (into h) -> add + RMSNorm (x = down + x2, h = next norm)
+// Above this many rows the GEMM layer chain runs q, k and v as separate GEMMs, and gate and up as two GEMMs +
+// fused_glu, instead of the grouped launches.  Measured on an H100 SXM (700 W), Llama-3-8B layer shapes (DESIGN §5.3):
+// the grouped QKV takes 0.54-0.89 x the separate launches from 256 to 2048 rows on Q8_0 but 1.17 x at 4096 and 1.12 x
+// at 8192 (Q4_K_M's q|k + v: 0.89 x at 256 rows, 1.09-1.15 x from 1024 up); the GLU epilogue takes 0.93-0.94 x at 1024
+// rows and 1.00-1.03 x from 2048 up.  Results are bit-identical either way.  A decode or verify step has at most 2048
+// rows, so only the prompt step reaches the separate launches.
+constexpr int GEMM_CHAIN_GROUPED_MAX_ROWS = 2048;
+
+// the linears of the GEMM layer chain: `rows` rows on the wgmma dequant GEMM (mrs_mmq_gguf_grouped).
+// whole_k: a row's result must not depend on the other rows of the launch, so K is never split (pdl | 2: a K split is
+// chosen from the row count and sums the partials in another order), and a single matrix above 64 rows takes the
+// plain ggml source of mrs_mmq_gguf, which runs faster than the one-matrix grouped source at prefill sizes and never
+// splits K there (tc_gemm.cuh splits only token tiles of up to 64 rows).
+struct GemmChain {
+  const mrs_llama_step *s;
+  int rows;
+  bool whole_k;
+  void *stream;
+
+  int32_t grouped(int type, int n, const void **w, const int32_t *n_rows, void **y, const void *x, int K, int glu) const {
+    return mrs_mmq_gguf_grouped(type, n, w, n_rows, y, x, rows, K, s->act_dtype, glu, whole_k ? s->pdl | 2 : s->pdl, stream);
+  }
+  // y = x W^T for the N-row matrix W
+  int32_t single(const mrs_qweight &W, int N, void *y, const void *x, int K) const {
+    if (whole_k && rows > 64) return mrs_mmq_gguf(W.ggml_type, W.data, x, y, rows, N, K, s->act_dtype, stream);
+    const void *w[1] = {W.data};
+    const int32_t n_rows[1] = {N};
+    void *yy[1] = {y};
+    return grouped(W.ggml_type, 1, w, n_rows, yy, x, K, 0);
+  }
+};
+
+// the GEMM layer chain's buffers, of c.rows rows each: gate_up [2, rows, inter] is read only above
+// GEMM_CHAIN_GROUPED_MAX_ROWS rows
+struct GemmChainBufs {
+  const int32_t *token_ids;
+  void *x, *x2, *h, *q, *k, *v, *attn_out, *act, *gate_up;
+};
+
+// The layer stack of the 9..256-sequence decode and verify steps and of the prompt step, up to the final norm in h.  The
+// norms are their own launches (the GEMM reads X through the TMA, unmodified), into the normed-activation buffer h:
+//   embedding gather -> RMSNorm; per layer:
+//   QKV (grouped: one launch, or q|k + v when attn_v has its own type; else three) -> attention(L) -> o GEMM (into h)
+//   -> add + RMSNorm (x2 = o + x, h = norm) -> gate|up GEMM with the GLU epilogue (act) -> down GEMM (into h)
+//   -> add + RMSNorm (x = down + x2, h = the next layer's norm, the final norm after the last layer)
 // The o and down GEMMs write into h, which the add + RMSNorm after them reads as its input and overwrites with the
-// norm: the norm kernel reads a row's input before its block-wide reduction and writes the row after it.
-// then the lm_head GEMM on h and argmax.  Every launch after the embedding gather and the first norm is a link of the
-// PDL chain when s->pdl is set.
-// q_len > 1 is a speculative verify step of the 9..256-sequence route: every row-wise launch covers batch * q_len rows
-// and the attention is mrs_paged_decode_fused_multi over the batch's sequences, as in llama_forward.  q_len == 1
-// issues exactly the decode step's launches.
-static int32_t llama_forward_gemm(const mrs_llama_step *s, int q_len, void *stream) {
-  const int dt = s->act_dtype, NS = s->batch, B = s->batch * q_len, H = s->hidden, pdl = s->pdl;
+// norm: the norm kernel reads a row's input before its block-wide reduction and writes the row after it.  Every launch
+// after the embedding gather and the first norm is a link of the PDL chain when s->pdl is set.  do_gemm == false
+// skips the linears (decode's skip_mask bit 1).
+template <class Attention>
+static int32_t gemm_layer_chain(const GemmChain &c, const GemmChainBufs &b, bool do_gemm, Attention attention) {
+  const mrs_llama_step *s = c.s;
+  const int dt = s->act_dtype, H = s->hidden, T = c.rows;
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool do_attn = !(s->skip_mask & 1), do_gemm = !(s->skip_mask & 2);
-  if (s->h == nullptr || (dt != MRS_F16 && dt != MRS_BF16)) return (int32_t)cudaErrorInvalidValue;
-  auto gemm = [&](int type, int n, const void **w, const int32_t *rows, void **y, const void *x, int K, int glu) {
-    return mrs_mmq_gguf_grouped(type, n, w, rows, y, x, B, K, dt, glu, pdl, stream);
-  };
+  const bool grouped = T <= GEMM_CHAIN_GROUPED_MAX_ROWS;
   auto add_rms = [&](const void *x, const void *res, const void *w, void *res_dst) {
-    mrs_add_rms_norm_pdl(x, res, w, res_dst, s->h, B, H, s->rms_eps, dt, pdl, stream);
+    mrs_add_rms_norm_pdl(x, res, w, res_dst, b.h, T, H, s->rms_eps, dt, s->pdl, c.stream);
   };
 
-  MRS_TRY(mrs_embedding_gather(s->tok_embd.ggml_type, s->tok_embd.data, H, s->token_ids, B, s->x, dt, stream));
-  if (dt == MRS_F16) mrs_rms_norm_f16(s->x, s->layers[0].attn_norm, s->h, B, H, s->rms_eps, (int64_t)stream);
-  else mrs_rms_norm_bf16(s->x, s->layers[0].attn_norm, s->h, B, H, s->rms_eps, (int64_t)stream);
+  MRS_TRY(mrs_embedding_gather(s->tok_embd.ggml_type, s->tok_embd.data, H, b.token_ids, T, b.x, dt, c.stream));
+  if (dt == MRS_F16) mrs_rms_norm_f16(b.x, s->layers[0].attn_norm, b.h, T, H, s->rms_eps, (int64_t)c.stream);
+  else mrs_rms_norm_bf16(b.x, s->layers[0].attn_norm, b.h, T, H, s->rms_eps, (int64_t)c.stream);
   for (int l = 0; l < s->n_layers; l++) {
     const mrs_llama_layer &L = s->layers[l];
     if (do_gemm) {
       const void *w[3] = {L.wq.data, L.wk.data, L.wv.data};
-      int32_t rows[3] = {nq, nkv, nkv};
-      void *y[3] = {s->q, s->k, s->v};
-      if (L.wq.ggml_type == L.wk.ggml_type && L.wk.ggml_type == L.wv.ggml_type) {
-        MRS_TRY(gemm(L.wq.ggml_type, 3, w, rows, y, s->h, H, 0));
-      } else if (L.wq.ggml_type == L.wk.ggml_type) {   // Q4_K_M keeps attn_v in Q6_K on some layers
-        MRS_TRY(gemm(L.wq.ggml_type, 2, w, rows, y, s->h, H, 0));
-        MRS_TRY(gemm(L.wv.ggml_type, 1, w + 2, rows + 2, y + 2, s->h, H, 0));
+      const int32_t rows[3] = {nq, nkv, nkv};
+      void *y[3] = {b.q, b.k, b.v};
+      if (grouped && L.wq.ggml_type == L.wk.ggml_type && L.wk.ggml_type == L.wv.ggml_type) {
+        MRS_TRY(c.grouped(L.wq.ggml_type, 3, w, rows, y, b.h, H, 0));
+      } else if (grouped && L.wq.ggml_type == L.wk.ggml_type) {   // Q4_K_M keeps attn_v in Q6_K on some layers
+        MRS_TRY(c.grouped(L.wq.ggml_type, 2, w, rows, y, b.h, H, 0));
+        MRS_TRY(c.single(L.wv, nkv, b.v, b.h, H));
       } else {
-        const int types[3] = {L.wq.ggml_type, L.wk.ggml_type, L.wv.ggml_type};
-        for (int m = 0; m < 3; m++) MRS_TRY(gemm(types[m], 1, w + m, rows + m, y + m, s->h, H, 0));
+        MRS_TRY(c.single(L.wq, nq, b.q, b.h, H));
+        MRS_TRY(c.single(L.wk, nkv, b.k, b.h, H));
+        MRS_TRY(c.single(L.wv, nkv, b.v, b.h, H));
       }
     }
-    if (do_attn && q_len > 1) {
-      MRS_TRY(mrs_paged_decode_fused_multi(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
-                                           s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
-                                           s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                                           s->block_valid_mask, s->attn_out, s->padded_tiles > NS ? s->tmp_v : nullptr,
-                                           s->padded_tiles > NS ? s->tmp_s : nullptr, s->attn_counters, NS, s->padded_tiles,
-                                           s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
-                                           pdl | (s->rope_neox ? 0 : 2), q_len, stream));
-    } else if (do_attn && s->fused_attention) {
-      MRS_TRY(mrs_paged_decode_fused(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
-                                     s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
-                                     s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                                     s->block_valid_mask, s->attn_out, s->padded_tiles > B ? s->tmp_v : nullptr,
-                                     s->padded_tiles > B ? s->tmp_s : nullptr, s->attn_counters, B, s->padded_tiles,
-                                     s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
-                                     pdl | (s->rope_neox ? 0 : 2), stream));
-    } else if (do_attn) {
-      rotary_embedding_positions(s->q, s->k, (void *)s->rope_cos, (void *)s->rope_sin, s->positions, s->rope_neox,
-                                 s->head_dim, B, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt,
-                                 (int64_t)stream);
-      reshape_and_cache_flashinfer(s->k, s->v, L.k_cache, L.v_cache, s->slot_mapping, B, s->n_kv_heads, s->head_dim,
-                                   s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
-      MRS_TRY(flashinfer_decode(s->q, L.k_cache, L.v_cache, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
-                                s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                                (const bool *)s->block_valid_mask, s->attn_out, s->padded_tiles > B ? s->tmp_v : nullptr,
-                                s->padded_tiles > B ? s->tmp_s : nullptr, B, s->padded_tiles, s->n_heads, s->n_kv_heads,
-                                s->head_dim, s->block_size, nq, s->head_dim, s->sm_scale, -1, 0.f, 1.f, 1.f,
-                                (uint32_t)dt, (uint32_t)dt, st));
-    }
+    MRS_TRY(attention(L));
     if (!do_gemm) continue;
-    {
-      const void *w[1] = {L.wo.data};
-      const int32_t rows[1] = {H};
-      void *y[1] = {s->h};
-      MRS_TRY(gemm(L.wo.ggml_type, 1, w, rows, y, s->attn_out, nq, 0));
-    }
-    add_rms(s->h, s->x, L.ffn_norm, s->x2);                                     // x2 = o + x ; h = norm(x2)
-    if (L.w_gate.ggml_type != L.w_up.ggml_type || L.w_gate.rows != L.w_up.rows) return (int32_t)cudaErrorInvalidValue;
-    {
+    MRS_TRY(c.single(L.wo, H, b.h, b.attn_out, nq));
+    add_rms(b.h, b.x, L.ffn_norm, b.x2);                                     // x2 = o + x ; h = norm(x2)
+    if (grouped) {
       const void *w[2] = {L.w_gate.data, L.w_up.data};
       const int32_t rows[2] = {L.w_gate.rows, L.w_up.rows};
-      void *y[2] = {s->act, nullptr};
-      MRS_TRY(gemm(L.w_gate.ggml_type, 2, w, rows, y, s->h, H, 1));
+      void *y[2] = {b.act, nullptr};
+      MRS_TRY(c.grouped(L.w_gate.ggml_type, 2, w, rows, y, b.h, H, 1));
+    } else {   // gate and up into the two halves of gate_up, then SiLU(gate) * up
+      const int I = L.w_gate.rows;
+      void *up = (uint8_t *)b.gate_up + (size_t)T * I * 2;
+      MRS_TRY(c.single(L.w_gate, I, b.gate_up, b.h, H));
+      MRS_TRY(c.single(L.w_up, I, up, b.h, H));
+      if (dt == MRS_F16) fused_glu_f16(b.gate_up, up, b.act, T, I, I, I, 0, (cudaStream_t)c.stream);
+      else fused_glu_bf16(b.gate_up, up, b.act, T, I, I, I, 0, (cudaStream_t)c.stream);
     }
-    {
-      const void *w[1] = {L.w_down.data};
-      const int32_t rows[1] = {H};
-      void *y[1] = {s->h};
-      MRS_TRY(gemm(L.w_down.ggml_type, 1, w, rows, y, s->act, L.w_down.cols, 0));
-    }
-    add_rms(s->h, s->x2, l + 1 < s->n_layers ? s->layers[l + 1].attn_norm : s->final_norm, s->x);   // x = down + x2 ; h = next norm(x)
+    MRS_TRY(c.single(L.w_down, H, b.h, b.act, L.w_down.cols));
+    add_rms(b.h, b.x2, l + 1 < s->n_layers ? s->layers[l + 1].attn_norm : s->final_norm, b.x);   // x = down + x2 ; h = next norm(x)
   }
-  if (do_gemm) {
-    const void *w[1] = {s->lm_head.data};
-    const int32_t rows[1] = {s->vocab};
-    void *y[1] = {s->logits};
-    MRS_TRY(gemm(s->lm_head.ggml_type, 1, w, rows, y, s->h, H, 0));
-  }
-  MRS_TRY(mrs_argmax(s->logits, B, s->vocab, dt, s->out_token, s->argmax_scratch, pdl, stream));
+  return 0;
+}
+
+// the decode step for 9..256 sequences: the reference's GgmlMatMul sends batches above 8 rows to MMQ, so the linears are
+// the wgmma dequant GEMM with the prefill GEMM's numerics: the GEMM layer chain over batch * q_len rows with the decode
+// attention, then the lm_head GEMM on h and argmax.  q_len > 1 is a speculative verify step of the 9..256-sequence route.
+static int32_t llama_forward_gemm(const mrs_llama_step *s, int q_len, void *stream) {
+  if (s->h == nullptr || (s->act_dtype != MRS_F16 && s->act_dtype != MRS_BF16)) return (int32_t)cudaErrorInvalidValue;
+  if (const int32_t e = check_model(s)) return e;
+  const bool do_attn = !(s->skip_mask & 1), do_gemm = !(s->skip_mask & 2);
+  const GemmChain c{s, s->batch * q_len, false, stream};
+  MRS_TRY(gemm_layer_chain(c, {s->token_ids, s->x, s->x2, s->h, s->q, s->k, s->v, s->attn_out, s->act, nullptr}, do_gemm,
+                           [&](const mrs_llama_layer &L) { return do_attn ? decode_attention(s, L, q_len, stream) : 0; }));
+  if (do_gemm) MRS_TRY(c.single(s->lm_head, s->vocab, s->logits, s->h, s->hidden));
+  MRS_TRY(mrs_argmax(s->logits, c.rows, s->vocab, s->act_dtype, s->out_token, s->argmax_scratch, s->pdl, stream));
   return (int32_t)cudaGetLastError();
 }
 
@@ -741,15 +724,8 @@ extern "C" int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len,
                          s->pdl, stream);
 }
 
-// Above this many rows the prompt step runs q, k and v as separate GEMMs, and gate and up as two GEMMs + fused_glu,
-// instead of the grouped launches.  Measured on an H100 SXM (700 W), Llama-3-8B layer shapes (DESIGN §5.3): the
-// grouped QKV takes 0.54-0.89 x the separate launches from 256 to 2048 rows on Q8_0 but 1.17 x at 4096 and 1.12 x at
-// 8192 (Q4_K_M's q|k + v: 0.89 x at 256 rows, 1.09-1.15 x from 1024 up); the GLU epilogue takes 0.93-0.94 x at 1024
-// rows and 1.00-1.03 x from 2048 up.  Results are bit-identical either way.
-constexpr int PREFILL_GROUPED_MAX_ROWS = 2048;
-
-// the prompt step over the packed rows of n sequences (contract: include/mrs_b200_model.h).  The layer chain is the one
-// of llama_forward_gemm over T rows; attention is the var-len prompt attention instead of the decode attention.
+// the prompt step over the packed rows of n sequences (contract: include/mrs_b200_model.h): the GEMM layer chain over T
+// rows with whole K, with the var-len prompt attention instead of the decode attention
 extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_llama_prefill *p, void *stream) {
   if (s == nullptr || p == nullptr) return (int32_t)cudaErrorInvalidValue;
   const int n = p->n_seqs, T = p->total_tokens, dt = s->act_dtype, H = s->hidden, pdl = s->pdl;
@@ -761,8 +737,7 @@ extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_lla
       p->cu_seqlens_q == nullptr || p->cu_seqlens_k == nullptr || p->x == nullptr || p->x2 == nullptr || p->h == nullptr ||
       p->q == nullptr || p->k == nullptr || p->v == nullptr || p->attn_out == nullptr || p->act == nullptr)
     return (int32_t)cudaErrorInvalidValue;
-  const bool grouped = T <= PREFILL_GROUPED_MAX_ROWS;
-  if (!grouped && p->gate_up == nullptr) return (int32_t)cudaErrorInvalidValue;
+  if (T > GEMM_CHAIN_GROUPED_MAX_ROWS && p->gate_up == nullptr) return (int32_t)cudaErrorInvalidValue;
   if (p->paged && (p->block_tables == nullptr || p->block_table_stride < 1 || p->num_blocks < 1)) return (int32_t)cudaErrorInvalidValue;
   if (p->lm_rows == 1 && (p->last_rows == nullptr || p->h_last == nullptr || p->logits == nullptr || p->out_token == nullptr ||
                           p->argmax_scratch == nullptr || (n <= 8 && p->q8_scratch == nullptr)))
@@ -770,47 +745,26 @@ extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_lla
   if (p->lm_rows == 2 && p->logits == nullptr) return (int32_t)cudaErrorInvalidValue;
   if (p->dest_rows != nullptr && (p->runner_token_ids == nullptr || p->runner_context_lens == nullptr))
     return (int32_t)cudaErrorInvalidValue;
+  if (const int32_t e = check_model(s)) return e;
+  // the lm_head of n <= 8 last rows: the reference-shaped MMVQ launcher of its type
+  void (*lm_mmvq)(const void *, const void *, void *, int, int, int, int, int, void *) = nullptr;
+  if (p->lm_rows == 1 && n <= 8) {
+#define MRS_PLAIN_CASE(TYPE, tag) \
+  case TYPE: lm_mmvq = dt == MRS_F16 ? launch_mmvq_gguf_##tag##_f16_plain : launch_mmvq_gguf_##tag##_bf16_plain; break;
+    switch (s->lm_head.ggml_type) {
+      MRS_PLAIN_CASE(MRS_Q4_0, q4_0) MRS_PLAIN_CASE(MRS_Q4_1, q4_1) MRS_PLAIN_CASE(MRS_Q5_0, q5_0)
+      MRS_PLAIN_CASE(MRS_Q5_1, q5_1) MRS_PLAIN_CASE(MRS_Q8_0, q8_0) MRS_PLAIN_CASE(MRS_Q2_K, q2_k)
+      MRS_PLAIN_CASE(MRS_Q3_K, q3_k) MRS_PLAIN_CASE(MRS_Q4_K, q4_k) MRS_PLAIN_CASE(MRS_Q5_K, q5_k)
+      MRS_PLAIN_CASE(MRS_Q6_K, q6_k)
+      default: return (int32_t)cudaErrorInvalidValue;
+    }
+#undef MRS_PLAIN_CASE
+  }
 
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
   cudaStream_t st = (cudaStream_t)stream;
-  // pdl | 2: K is never split, so a sequence's rows come out the same whatever other rows share the launch
-  auto gemm = [&](int type, int nm, const void **w, const int32_t *rows, void **y, const void *x, int M, int K, int glu) {
-    return mrs_mmq_gguf_grouped(type, nm, w, rows, y, x, M, K, dt, glu, pdl | 2, stream);
-  };
-  // one matrix: above 64 rows the plain ggml source of mrs_mmq_gguf, which runs faster than the grouped source at
-  // prefill sizes and never splits K there (tc_gemm.cuh splits only token tiles of up to 64 rows); up to 64 rows the
-  // grouped launch with whole K.  Same results either way.
-  auto linear = [&](const mrs_qweight &W, int N, void *y, const void *x, int M, int K) -> int32_t {
-    if (M > 64) return mrs_mmq_gguf(W.ggml_type, W.data, x, y, M, N, K, dt, stream);
-    const void *w[1] = {W.data};
-    const int32_t rows[1] = {N};
-    void *yy[1] = {y};
-    return gemm(W.ggml_type, 1, w, rows, yy, x, M, K, 0);
-  };
-  auto add_rms = [&](const void *x, const void *res, const void *w, void *res_dst) {
-    mrs_add_rms_norm_pdl(x, res, w, res_dst, p->h, T, H, s->rms_eps, dt, pdl, stream);
-  };
-
-  MRS_TRY(mrs_embedding_gather(s->tok_embd.ggml_type, s->tok_embd.data, H, p->token_ids, T, p->x, dt, stream));
-  if (dt == MRS_F16) mrs_rms_norm_f16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
-  else mrs_rms_norm_bf16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
-  for (int l = 0; l < s->n_layers; l++) {
-    const mrs_llama_layer &L = s->layers[l];
-    {
-      const void *w[3] = {L.wq.data, L.wk.data, L.wv.data};
-      int32_t rows[3] = {nq, nkv, nkv};
-      void *y[3] = {p->q, p->k, p->v};
-      if (grouped && L.wq.ggml_type == L.wk.ggml_type && L.wk.ggml_type == L.wv.ggml_type) {
-        MRS_TRY(gemm(L.wq.ggml_type, 3, w, rows, y, p->h, T, H, 0));
-      } else if (grouped && L.wq.ggml_type == L.wk.ggml_type) {   // Q4_K_M keeps attn_v in Q6_K on some layers
-        MRS_TRY(gemm(L.wq.ggml_type, 2, w, rows, y, p->h, T, H, 0));
-        MRS_TRY(linear(L.wv, nkv, p->v, p->h, T, H));
-      } else {
-        MRS_TRY(linear(L.wq, nq, p->q, p->h, T, H));
-        MRS_TRY(linear(L.wk, nkv, p->k, p->h, T, H));
-        MRS_TRY(linear(L.wv, nkv, p->v, p->h, T, H));
-      }
-    }
+  const GemmChain c{s, T, true, stream};
+  auto attention = [&](const mrs_llama_layer &L) -> int32_t {
     rotary_embedding_positions(p->q, p->k, (void *)s->rope_cos, (void *)s->rope_sin, (void *)p->positions, s->rope_neox,
                                s->head_dim, T, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt,
                                (int64_t)stream);
@@ -819,58 +773,29 @@ extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_lla
                                     s->n_kv_heads, s->head_dim, nq, nkv, nq, s->sm_scale, 1, -1, 0.f, (uint32_t)dt, stream));
       reshape_and_cache_flashinfer(p->k, p->v, L.k_cache, L.v_cache, (int64_t *)p->slot_mapping, T, s->n_kv_heads,
                                    s->head_dim, s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
-    } else {           // the new rows join the cached ones in the cache, then attend over the pages
-      reshape_and_cache_flashinfer(p->k, p->v, L.k_cache, L.v_cache, (int64_t *)p->slot_mapping, T, s->n_kv_heads,
-                                   s->head_dim, s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
-      MRS_TRY(mrs_prefill_attention_paged(p->q, L.k_cache, L.v_cache, p->attn_out, p->block_tables, p->block_table_stride,
-                                          p->cu_seqlens_q, p->cu_seqlens_k, n, T, p->max_q_len, p->max_kv_len,
-                                          p->num_blocks, s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, nq, nq,
-                                          s->sm_scale, 1, -1, 0.f, (uint32_t)dt, stream));
+      return 0;
     }
-    MRS_TRY(linear(L.wo, H, p->h, p->attn_out, T, nq));
-    add_rms(p->h, p->x, L.ffn_norm, p->x2);                                     // x2 = o + x ; h = norm(x2)
-    if (L.w_gate.ggml_type != L.w_up.ggml_type || L.w_gate.rows != L.w_up.rows) return (int32_t)cudaErrorInvalidValue;
-    if (grouped) {
-      const void *w[2] = {L.w_gate.data, L.w_up.data};
-      const int32_t rows[2] = {L.w_gate.rows, L.w_up.rows};
-      void *y[2] = {p->act, nullptr};
-      MRS_TRY(gemm(L.w_gate.ggml_type, 2, w, rows, y, p->h, T, H, 1));
-    } else {   // gate and up into the two halves of gate_up, then SiLU(gate) * up
-      const int I = L.w_gate.rows;
-      void *up = (uint8_t *)p->gate_up + (size_t)T * I * 2;
-      MRS_TRY(linear(L.w_gate, I, p->gate_up, p->h, T, H));
-      MRS_TRY(linear(L.w_up, I, up, p->h, T, H));
-      if (dt == MRS_F16) fused_glu_f16(p->gate_up, up, p->act, T, I, I, I, 0, st);
-      else fused_glu_bf16(p->gate_up, up, p->act, T, I, I, I, 0, st);
-    }
-    MRS_TRY(linear(L.w_down, H, p->h, p->act, T, L.w_down.cols));
-    add_rms(p->h, p->x2, l + 1 < s->n_layers ? s->layers[l + 1].attn_norm : s->final_norm, p->x);   // x = down + x2 ; h = next norm(x)
-  }
+    // the new rows join the cached ones in the cache, then attend over the pages
+    reshape_and_cache_flashinfer(p->k, p->v, L.k_cache, L.v_cache, (int64_t *)p->slot_mapping, T, s->n_kv_heads,
+                                 s->head_dim, s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
+    return mrs_prefill_attention_paged(p->q, L.k_cache, L.v_cache, p->attn_out, p->block_tables, p->block_table_stride,
+                                       p->cu_seqlens_q, p->cu_seqlens_k, n, T, p->max_q_len, p->max_kv_len, p->num_blocks,
+                                       s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, nq, nq, s->sm_scale, 1, -1,
+                                       0.f, (uint32_t)dt, stream);
+  };
+  MRS_TRY(gemm_layer_chain(c, {p->token_ids, p->x, p->x2, p->h, p->q, p->k, p->v, p->attn_out, p->act, p->gate_up}, true,
+                           attention));
   if (p->lm_rows == 2) {
-    MRS_TRY(linear(s->lm_head, s->vocab, p->logits, p->h, T, H));
+    MRS_TRY(c.single(s->lm_head, s->vocab, p->logits, p->h, H));
   } else if (p->lm_rows == 1) {
     last_row_gather_kernel<<<n, 128, 0, st>>>((const uint4 *)p->h, p->last_rows, (uint4 *)p->h_last, H / 8);
     if (n <= 8) {    // the reference's GgufMatMul at 1..8 rows: Q8_1 activations + MMVQ (fast_mmvq plain)
       const int kpad = (H + 511) / 512 * 512;
       if (dt == MRS_F16) launch_mmvq_gguf_quantize_q8_1_f16(p->h_last, p->q8_scratch, H, kpad, n, stream);
       else launch_mmvq_gguf_quantize_q8_1_bf16(p->h_last, p->q8_scratch, H, kpad, n, stream);
-      const void *W = s->lm_head.data;
-      const int V = s->vocab, sy = kpad / 32;
-#define MRS_PLAIN_CASE(TYPE, tag)                                                                        \
-  case TYPE:                                                                                             \
-    if (dt == MRS_F16) launch_mmvq_gguf_##tag##_f16_plain(W, p->q8_scratch, p->logits, H, V, sy, V, n, stream); \
-    else launch_mmvq_gguf_##tag##_bf16_plain(W, p->q8_scratch, p->logits, H, V, sy, V, n, stream);            \
-    break;
-      switch (s->lm_head.ggml_type) {
-        MRS_PLAIN_CASE(MRS_Q4_0, q4_0) MRS_PLAIN_CASE(MRS_Q4_1, q4_1) MRS_PLAIN_CASE(MRS_Q5_0, q5_0)
-        MRS_PLAIN_CASE(MRS_Q5_1, q5_1) MRS_PLAIN_CASE(MRS_Q8_0, q8_0) MRS_PLAIN_CASE(MRS_Q2_K, q2_k)
-        MRS_PLAIN_CASE(MRS_Q3_K, q3_k) MRS_PLAIN_CASE(MRS_Q4_K, q4_k) MRS_PLAIN_CASE(MRS_Q5_K, q5_k)
-        MRS_PLAIN_CASE(MRS_Q6_K, q6_k)
-        default: return (int32_t)cudaErrorInvalidValue;
-      }
-#undef MRS_PLAIN_CASE
+      lm_mmvq(s->lm_head.data, p->q8_scratch, p->logits, H, s->vocab, kpad / 32, s->vocab, n, stream);
     } else {         // 9 and more rows: the dequant GEMM (the reference's MMQ branch)
-      MRS_TRY(linear(s->lm_head, s->vocab, p->logits, p->h_last, n, H));
+      MRS_TRY((GemmChain{s, n, true, stream}.single(s->lm_head, s->vocab, p->logits, p->h_last, H)));
     }
     MRS_TRY(mrs_argmax(p->logits, n, s->vocab, dt, p->out_token, p->argmax_scratch, pdl, stream));
     if (p->dest_rows != nullptr)

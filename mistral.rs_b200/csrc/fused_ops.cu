@@ -98,16 +98,8 @@ static void launch_glu(const void *a, const void *b, void *out, uint32_t rows, u
                        int act, cudaStream_t st, int pdl = 0) {
   if (rows == 0 || cols == 0) return;
   const uint64_t n = (uint64_t)rows * cols;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)((n + 255) / 256));
-  cfg.blockDim = dim3(256);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, glu_kernel<T>, (const T *)a, (const T *)b, (T *)out, cols, as, bs, n, act, pdl);
+  launch_pdl(glu_kernel<T>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, pdl, (const T *)a, (const T *)b, (T *)out,
+             cols, as, bs, n, act, pdl);
 }
 
 // ------------------------------------------------------------------ RMSNorm
@@ -153,16 +145,8 @@ static void launch_rms(const void *x, const void *res, const void *w, void *sum_
                        float eps, cudaStream_t st, int pdl = 0) {
   if (rows <= 0 || cols <= 0) return;
   const int block = cols < 1024 ? 128 : 512;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(rows);
-  cfg.blockDim = dim3(block);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, rms_norm_kernel<T>, (const T *)x, (const T *)res, (const T *)w, (T *)sum_out, (T *)out, cols, eps, pdl);
+  launch_pdl(rms_norm_kernel<T>, dim3(rows), dim3(block), 0, st, pdl, (const T *)x, (const T *)res, (const T *)w,
+             (T *)sum_out, (T *)out, cols, eps, pdl);
 }
 
 // Per-head RMSNorm of a strided [B, H, S, D] view into a contiguous [B, H, S, D] tensor (QK-norm of

@@ -11,7 +11,6 @@
 #include "common.cuh"
 #include "mrs_b200_model.h"
 
-#include <stdio.h>
 
 extern "C" int32_t mrs_w4a16_gemm(const void *x, const void *w_tiles, const void *scales, const int32_t *qzeros, void *y,
                                   int32_t M, int32_t K, int32_t N, int32_t group, int32_t dtype, int32_t scale_perm,
@@ -66,15 +65,6 @@ __global__ void dense_embedding_kernel(const uint4 *__restrict__ table, int cols
   for (int i = threadIdx.x; i < cols8; i += blockDim.x) out[(int64_t)blockIdx.x * cols8 + i] = table[row * cols8 + i];
 }
 }  // namespace mrs
-
-#define MRS_TRY(expr)                                                \
-  do {                                                               \
-    const int _e = (int)(expr);                                      \
-    if (_e != 0) {                                                   \
-      fprintf(stderr, "mrs_b200: %s -> cudaError %d\n", #expr, _e);  \
-      return _e;                                                     \
-    }                                                                \
-  } while (0)
 
 extern "C" int32_t mrs_w4a16_gemm_pdl(const void *x, const void *w_tiles, const void *scales, const int32_t *qzeros, void *y,
                                       int32_t M, int32_t K, int32_t N, int32_t group, int32_t dtype, int32_t scale_perm,

@@ -653,17 +653,7 @@ static cudaError_t launch_one(MmvqParams p, cudaStream_t stream) {
   // the attribute is per device (context): set it on every launch — it is cheap, and a process-wide
   // "already set" flag would leave the second GPU of a multi-device process at the 48 KB default
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3((NCW + 1) * 32);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = p.pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, p);
+  return launch_pdl(kern, dim3(grid), dim3((NCW + 1) * 32), smem, stream, p.pdl, p);
 }
 
 template <int T> static bool rows_aligned(const MmvqParams &p) {
@@ -705,17 +695,7 @@ static cudaError_t launch_dual(MmvqParams pa, MmvqParams pb, cudaStream_t stream
   }
   auto kern = mmvq_dual_kernel<T1, T2>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(ga + gb);
-  cfg.blockDim = dim3(9 * 32);
-  cfg.dynamicSmemBytes = sma > smb ? sma : smb;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pa.pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, pa, pb, ga);
+  return launch_pdl(kern, dim3(ga + gb), dim3(9 * 32), sma > smb ? sma : smb, stream, pa.pdl, pa, pb, ga);
 }
 
 // supported type pairs of the two-type launch (the k-quant "M" recipes: attn_v one step up)

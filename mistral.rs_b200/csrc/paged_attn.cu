@@ -606,13 +606,7 @@ static int g_pa_flags = 0;   // bit 0: keep HND decode on the SIMT kernel (A/B, 
 template <typename K>
 static cudaError_t launch_pa(K kern, dim3 grid, const PagedParams &p, cudaStream_t st, size_t dyn_smem, int threads = PA_THREADS) {
   if (dyn_smem > 0) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = dyn_smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = p.pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, p);
+  return launch_pdl(kern, grid, dim3(threads), dyn_smem, st, p.pdl, p);
 }
 
 // the split tiles of one sequence as one thread-block cluster (merge through DSMEM).  Returns false, launching nothing,
@@ -886,6 +880,38 @@ MRS_PAGED(bf16, 1u)
 MRS_PAGED(f32, 2u)
 
 // ---------------------------------------------------------------- native fused decode attention
+// the PagedParams of the fused decode entry points; the split-KV tiles (tmp_o != nullptr) are used only when the plan
+// has more tiles than sequences
+static PagedParams fused_decode_params(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
+                                       const void *rope_cos, const void *rope_sin, const int32_t *positions,
+                                       const int64_t *slot_mapping, const int32_t *kv_indptr, const int32_t *kv_indices,
+                                       const int32_t *kv_last_page_len, const int32_t *request_indices,
+                                       const int32_t *kv_tile_indices, const int32_t *o_indptr,
+                                       const int32_t *kv_chunk_size_ptr, const uint8_t *block_valid_mask, void *o,
+                                       void *tmp_v, float *tmp_s, int32_t *counters, int32_t batch_size,
+                                       int32_t padded_batch_size, int32_t num_qo_heads, int32_t num_kv_heads,
+                                       int32_t head_size, int32_t page_size, float sm_scale, int32_t pdl,
+                                       int64_t q_stride_n, int64_t kv_new_stride) {
+  PagedParams p = {};
+  p.q = q; p.kc = key_cache; p.vc = value_cache; p.out = o;
+  const bool split = tmp_v != nullptr && padded_batch_size > batch_size;
+  p.tmp_o = split ? tmp_v : nullptr; p.tmp_lse = split ? tmp_s : nullptr;
+  if (split) {
+    p.request_indices = request_indices; p.kv_tile_indices = kv_tile_indices;
+    p.block_valid_mask = block_valid_mask; p.kv_chunk_size_ptr = kv_chunk_size_ptr;
+  }
+  p.kv_indptr = kv_indptr; p.kv_indices = kv_indices; p.kv_last_page_len = kv_last_page_len;
+  p.kv_block_stride = (int64_t)num_kv_heads * page_size * head_size; p.kv_head_stride = (int64_t)page_size * head_size;
+  p.num_heads = num_qo_heads; p.num_kv_heads = num_kv_heads; p.page_size = page_size;
+  p.q_stride_n = q_stride_n; p.q_stride_h = head_size; p.sm_scale = sm_scale;
+  p.window_left = -1; p.pdl = pdl & 1; p.rope_interleaved = (pdl >> 1) & 1;
+  p.k_new = k_new; p.v_new = v_new; p.kv_new_stride = kv_new_stride;
+  p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.positions = positions; p.slot_mapping = slot_mapping;
+  p.o_indptr = o_indptr; p.counters = counters; p.batch_size = batch_size;
+  p.k_scale = 1.f; p.v_scale = 1.f;
+  return p;
+}
+
 // RoPE(q, k_new) + KV-cache write + paged decode attention + split-KV merge in ONE launch over
 // the HND cache.  q [B, H*D], k_new/v_new [B, KVH*D] are the raw QKV GEMV outputs; cos/sin
 // [max_pos, D/2]; positions [B] i32; slot_mapping [B] i64; counters: zeroed int32
@@ -906,24 +932,12 @@ extern "C" int32_t mrs_paged_decode_fused_strided(void *q, void *k_new, void *v_
                                           int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
                                           int64_t q_stride_n, int64_t kv_new_stride, void *stream) {
   if (dtype != 0 && dtype != 1) return (int32_t)cudaErrorInvalidValue;
-  PagedParams p = {};
-  p.q = q; p.kc = key_cache; p.vc = value_cache; p.out = o;
-  const bool split = tmp_v != nullptr && padded_batch_size > batch_size;
-  p.tmp_o = split ? tmp_v : nullptr; p.tmp_lse = split ? tmp_s : nullptr;
-  if (split) {
-    p.request_indices = request_indices; p.kv_tile_indices = kv_tile_indices;
-    p.block_valid_mask = block_valid_mask; p.kv_chunk_size_ptr = kv_chunk_size_ptr;
-  }
-  p.kv_indptr = kv_indptr; p.kv_indices = kv_indices; p.kv_last_page_len = kv_last_page_len;
-  p.kv_block_stride = (int64_t)num_kv_heads * page_size * head_size; p.kv_head_stride = (int64_t)page_size * head_size;
-  p.num_heads = num_qo_heads; p.num_kv_heads = num_kv_heads; p.page_size = page_size;
-  p.q_stride_n = q_stride_n; p.q_stride_h = head_size; p.sm_scale = sm_scale;
-  p.window_left = -1; p.pdl = pdl & 1; p.rope_interleaved = (pdl >> 1) & 1;
-  p.k_new = k_new; p.v_new = v_new; p.kv_new_stride = kv_new_stride;
-  p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.positions = positions; p.slot_mapping = slot_mapping;
-  p.o_indptr = o_indptr; p.counters = counters; p.batch_size = batch_size;
-  p.k_scale = 1.f; p.v_scale = 1.f;
-  const int tiles = split ? padded_batch_size : batch_size;
+  const PagedParams p = fused_decode_params(q, k_new, v_new, key_cache, value_cache, rope_cos, rope_sin, positions,
+                                            slot_mapping, kv_indptr, kv_indices, kv_last_page_len, request_indices,
+                                            kv_tile_indices, o_indptr, kv_chunk_size_ptr, block_valid_mask, o, tmp_v, tmp_s,
+                                            counters, batch_size, padded_batch_size, num_qo_heads, num_kv_heads, head_size,
+                                            page_size, sm_scale, pdl, q_stride_n, kv_new_stride);
+  const int tiles = p.tmp_o != nullptr ? padded_batch_size : batch_size;
   const cudaError_t e = (dtype == 0) ? launch_decode<__half, __half, 1, true>(p, head_size, tiles, (cudaStream_t)stream)
                                      : launch_decode<__nv_bfloat16, __nv_bfloat16, 1, true>(p, head_size, tiles, (cudaStream_t)stream);
   if (e != cudaSuccess) fprintf(stderr, "mrs_b200: mrs_paged_decode_fused failed: %s\n", cudaGetErrorString(e));
@@ -966,25 +980,14 @@ extern "C" int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_ne
   if ((dtype != 0 && dtype != 1) || (head_size != 64 && head_size != 128) || q_len < 1 || q_len > 8 || num_kv_heads < 1 ||
       num_qo_heads % num_kv_heads)
     return (int32_t)cudaErrorInvalidValue;
-  PagedParams p = {};
-  p.q = q; p.kc = key_cache; p.vc = value_cache; p.out = o;
-  const bool split = tmp_v != nullptr && padded_batch_size > batch_size;
-  p.tmp_o = split ? tmp_v : nullptr; p.tmp_lse = split ? tmp_s : nullptr;
-  if (split) {
-    p.request_indices = request_indices; p.kv_tile_indices = kv_tile_indices;
-    p.block_valid_mask = block_valid_mask; p.kv_chunk_size_ptr = kv_chunk_size_ptr;
-  }
-  p.kv_indptr = kv_indptr; p.kv_indices = kv_indices; p.kv_last_page_len = kv_last_page_len;
-  p.kv_block_stride = (int64_t)num_kv_heads * page_size * head_size; p.kv_head_stride = (int64_t)page_size * head_size;
-  p.num_heads = num_qo_heads; p.num_kv_heads = num_kv_heads; p.page_size = page_size;
-  p.q_stride_n = (int64_t)num_qo_heads * head_size; p.q_stride_h = head_size; p.sm_scale = sm_scale;
-  p.window_left = -1; p.pdl = pdl & 1; p.rope_interleaved = (pdl >> 1) & 1;
-  p.k_new = k_new; p.v_new = v_new; p.kv_new_stride = (int64_t)num_kv_heads * head_size;
-  p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.positions = positions; p.slot_mapping = slot_mapping;
-  p.o_indptr = o_indptr; p.counters = counters; p.batch_size = batch_size;
-  p.k_scale = 1.f; p.v_scale = 1.f;
+  PagedParams p = fused_decode_params(q, k_new, v_new, key_cache, value_cache, rope_cos, rope_sin, positions, slot_mapping,
+                                      kv_indptr, kv_indices, kv_last_page_len, request_indices, kv_tile_indices,
+                                      o_indptr, kv_chunk_size_ptr, block_valid_mask, o, tmp_v, tmp_s, counters,
+                                      batch_size, padded_batch_size, num_qo_heads, num_kv_heads, head_size,
+                                      page_size, sm_scale, pdl, (int64_t)num_qo_heads * head_size,
+                                      (int64_t)num_kv_heads * head_size);
   p.q_len = q_len;
-  const int tiles = split ? padded_batch_size : batch_size;
+  const int tiles = p.tmp_o != nullptr ? padded_batch_size : batch_size;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e;
   if (dtype == 0) e = head_size == 64 ? launch_decode_multi<__half, 64>(p, tiles, st) : launch_decode_multi<__half, 128>(p, tiles, st);

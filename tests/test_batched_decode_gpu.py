@@ -297,6 +297,27 @@ def test_context_overflow_freezes_one_sequence(cuda):
         assert np.abs(got[b] - want).max() / np.abs(want).max() <= Q8_0_LOGIT_TOL, b
 
 
+@pytest.mark.gpu
+@pytest.mark.parametrize("B", [1, 16])
+def test_decode_step_rejects_mismatched_gate_up(cuda, B):
+    """A last layer whose w_up has another ggml type than its w_gate gives cudaErrorInvalidValue before any launch, on
+    the GEMV route (B = 1) and the GEMM route (B = 16): no cache row and no logit is written."""
+    w = M.LlamaWeights(M.LlamaConfig.tiny_test(quant="q8_0", n_layers=2), cuda, dtype=torch.bfloat16)
+    run = M.LlamaRunner(w, batch=B, max_ctx=64)
+    run.set_tokens(list(range(1, B + 1)))
+    run.advance()
+    layers = (M._Layer * len(run._layers)).from_buffer_copy(run._layers)
+    layers[-1].w_up.ggml_type = GGML["q4_0"]
+    s = M._Step.from_buffer_copy(run.step_struct)
+    s.layers = ctypes.cast(layers, ctypes.POINTER(M._Layer))
+    torch.cuda.synchronize()
+    rc = lib().mrs_llama_decode_step(ctypes.byref(s), run._stream())
+    torch.cuda.synchronize()
+    assert rc == 1, rc
+    assert all(int(c.abs().sum()) == 0 for c in run.k_cache + run.v_cache)
+    assert int(run.logits().abs().sum()) == 0
+
+
 # ---------------------------------------------------------------- argument checks (no GPU)
 def test_decode_step_rejects_bad_batch():
     L = lib()

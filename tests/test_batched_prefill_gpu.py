@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import oracle
-from mistralrs_b200 import kv_index, lib
+from mistralrs_b200 import GGML, kv_index, lib
 from mistralrs_b200 import model as M
 from oracle.model import OracleLlama
 
@@ -267,7 +267,7 @@ def test_llama3_8b_shapes_batched_prefill(cuda):
 # ---------------------------------------------------------------- the C entry's rejections
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", ["n0", "n257", "t_lt_n", "null_x", "null_tables", "dtype", "tp", "lm_rows", "dest_rows",
-                                  "null_q8", "paged2"])
+                                  "null_q8", "paged2", "gate_up_type", "lm_head_type"])
 def test_prefill_step_rejects(cuda, case):
     """Each bad field alone gives cudaErrorInvalidValue (1) before anything is launched: the caches stay untouched."""
     w = M.LlamaWeights(_cfg("q8_0", "bf16"), cuda, dtype=torch.bfloat16)
@@ -298,6 +298,12 @@ def test_prefill_step_rejects(cuda, case):
         p.q8_scratch = None
     elif case == "paged2":
         p.paged = 2
+    elif case == "gate_up_type":      # only the last layer is wrong: the earlier layers must not run either
+        layers = (M._Layer * len(pre._layers)).from_buffer_copy(pre._layers)
+        layers[-1].w_up.ggml_type = GGML["q4_0"]
+        s.layers = ctypes.cast(layers, ctypes.POINTER(M._Layer))
+    elif case == "lm_head_type":      # no MMVQ launcher for the n <= 8 lm_head
+        s.lm_head.ggml_type = GGML["q8_1"]
     torch.cuda.synchronize()
     rc = lib().mrs_llama_prefill_step(ctypes.byref(s), ctypes.byref(p), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     torch.cuda.synchronize()
