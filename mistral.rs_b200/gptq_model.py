@@ -16,8 +16,8 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from . import kv_index, lib
-from .model import rope_tables, runner_split_pages
+from . import lib
+from .model import PagedDecodeRunner, _point, check_runner_args, rope_tables, runner_split_pages
 
 
 @dataclass
@@ -146,29 +146,17 @@ class GptqWeights:
         return (tiles, scales, K, N)
 
 
-class GptqRunner:
-    """KV cache + scratch + per-step metadata for a decode batch; drives mrs_gptq_decode_step."""
+class GptqRunner(PagedDecodeRunner):
+    """KV cache + scratch + per-step metadata for a decode batch; drives mrs_gptq_decode_step.  The vLLM cache layout
+    runs the unsplit attention plan."""
 
     def __init__(self, weights: GptqWeights, batch=32, max_ctx=512, cache_layout="hnd", sm_count=132):
-        cfg, dev, dt = weights.cfg, weights.device, weights.dtype
-        self.w, self.cfg, self.dev, self.dt, self.B = weights, cfg, dev, dt, batch
+        check_runner_args(batch)
+        cfg = weights.cfg
+        super().__init__(weights, batch, max_ctx, runner_split_pages(cfg.block_size, batch, cfg.n_kv_heads, max_ctx, sm_count)
+                         if cache_layout == "hnd" else 0)
+        batch, dev, dt, nb = self.B, self.dev, self.dt, self.B * self.max_blocks + 1
         bs, D, KVH, NH, H = cfg.block_size, cfg.head_dim, cfg.n_kv_heads, cfg.n_heads, cfg.hidden
-        self.max_blocks = -(-max_ctx // bs)
-        nb = batch * self.max_blocks + 1
-        self.pool = kv_index.BlockPool(nb)
-        self.tables = [self.pool.get_new_blocks(self.max_blocks) for _ in range(batch)]
-        self.block_tables = torch.tensor(self.tables, dtype=torch.int32, device=dev)
-        self.context_lens = torch.zeros(batch, dtype=torch.int32, device=dev)
-        self.error_flag = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.split_pages = runner_split_pages(bs, batch, KVH, max_ctx, sm_count)
-        self.padded_tiles = batch * -(-self.max_blocks // self.split_pages)
-        if self.padded_tiles <= batch or cache_layout != "hnd":
-            self.split_pages, self.padded_tiles = 0, batch
-        z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=dev)
-        self.meta = dict(token_ids=z(batch), positions=z(batch), slot_mapping=z(batch, d=torch.int64), kv_indptr=z(batch + 1),
-                         kv_indices=z(batch * self.max_blocks), kv_last_page_len=z(batch), request_indices=z(self.padded_tiles),
-                         kv_tile_indices=z(self.padded_tiles), o_indptr=z(batch + 1), kv_chunk_size=z(1),
-                         block_valid_mask=z(self.padded_tiles, d=torch.uint8))
         a = lambda *s: torch.zeros(*s, dtype=dt, device=dev)
         nq, nkv = NH * D, KVH * D
         self.buf = dict(x=a(batch, H), x2=a(batch, H), h=a(batch, H), qkv=a(batch, nq + 2 * nkv), attn_out=a(batch, nq),
@@ -200,53 +188,10 @@ class GptqRunner:
         s.layers = ctypes.cast(self._layers, ctypes.POINTER(_Layer))
         s.tok_embd, s.lm_head, s.final_norm = weights.tok_embd.data_ptr(), weights.lm_head.data_ptr(), weights.final_norm.data_ptr()
         s.rope_cos, s.rope_sin = weights.rope_cos.data_ptr(), weights.rope_sin.data_ptr()
-        for n, t in self.meta.items():
-            setattr(s, n, t.data_ptr())
-        s.block_tables, s.context_lens = self.block_tables.data_ptr(), self.context_lens.data_ptr()
-        for n, t in self.buf.items():
-            setattr(s, n, t.data_ptr())
-        self.step_struct, self.graph = s, None
-        self.max_ctx = min(self.max_blocks * bs, cfg.max_pos)
-
-    def _stream(self):
-        return ctypes.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
-
-    def advance(self):
-        m = self.meta
-        rc = lib().mrs_decode_advance(ctypes.c_void_p(self.block_tables.data_ptr()), ctypes.c_int(self.max_blocks),
-                                      ctypes.c_void_p(self.context_lens.data_ptr()), ctypes.c_int(self.B),
-                                      ctypes.c_int(self.cfg.block_size), ctypes.c_int(self.split_pages),
-                                      ctypes.c_int(self.padded_tiles), *[ctypes.c_void_p(m[k].data_ptr()) for k in
-                                      ("positions", "slot_mapping", "kv_indptr", "kv_indices", "kv_last_page_len",
-                                       "request_indices", "kv_tile_indices", "o_indptr", "kv_chunk_size", "block_valid_mask")],
-                                      ctypes.c_int(self.cfg.max_pos), ctypes.c_void_p(self.error_flag.data_ptr()), self._stream())
-        assert rc == 0, rc
+        _point(s, self.meta, dict(block_tables=self.block_tables, context_lens=self.context_lens), self.buf)
+        self.step_struct = s
 
     def forward(self):
         rc = lib().mrs_gptq_decode_step(ctypes.byref(self.step_struct), self._stream())
         if rc != 0:
             raise RuntimeError(f"mrs_gptq_decode_step failed: cudaError {rc}")
-
-    def step(self):
-        self.advance()
-        self.forward()
-
-    def reset(self, context_len=0):
-        self.context_lens.fill_(context_len)
-        self.error_flag.zero_()
-
-    def capture(self):
-        self.step(); self.reset()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self.step()
-        self.reset()
-        self.graph = g
-        return g
-
-    def set_tokens(self, ids):
-        self.meta["token_ids"].copy_(torch.as_tensor(ids, dtype=torch.int32, device=self.dev))
-
-    def logits(self):
-        return self.buf["logits"]

@@ -236,42 +236,52 @@ def compute_n_kv_groups(total_kv_heads: int, n_heads: int, world: int) -> int:
 class LlamaWeights:
     """Synthetic device-resident weights (optionally one tensor-parallel shard)."""
 
+    # the quantized tensors of a layer and how tensor parallelism splits them (see _shard)
+    GGUF_NAMES = {"attn_q": "col", "attn_k": "kv", "attn_v": "kv", "attn_output": "row", "ffn_gate": "col",
+                  "ffn_up": "col", "ffn_down": "row"}
+
     def __init__(self, cfg: LlamaConfig, device, dtype=torch.bfloat16, tp_rank=0, tp_size=1, keep_host=False, fast_synth=False):
         """fast_synth: generate the (shard-shaped) blocks on the device with torch's RNG instead of numpy
         PCG64 on the host — same distribution, not the SURVEY §8(d) byte stream; for throughput runs of
         large models (config 3's 8 GB, config 5's 40 GB) where no oracle comparison is made."""
-        self.cfg, self.device, self.dtype = cfg, device, dtype
-        self.tp_rank, self.tp_size = tp_rank, tp_size
-        self.fast_synth = bool(fast_synth)
         if fast_synth and keep_host:
             raise ValueError("fast_synth weights have no host copy")
-        self.host = {} if keep_host else None
+        self._setup(cfg, device, dtype, tp_rank, tp_size, keep_host)
+        self.fast_synth = bool(fast_synth)
         H, I = cfg.hidden, cfg.inter
+        if I % (tp_size * 256):
+            raise ValueError("tensor-parallel size must divide the intermediate size in 256-wide slices")
         nq, nkv = cfg.n_heads * cfg.head_dim, cfg.n_kv_heads * cfg.head_dim
-        assert cfg.n_heads % tp_size == 0 and I % (tp_size * 256) == 0
+        shape = {"attn_q": (nq, H), "attn_k": (nkv, H), "attn_v": (nkv, H), "attn_output": (H, nq), "ffn_gate": (I, H),
+                 "ffn_up": (I, H), "ffn_down": (H, I), "token_embd": (cfg.vocab, H), "output": (cfg.vocab, H)}
+        self._load(lambda l, name, kind: self._qtensor(l, name, *shape[name], kind), self._norm)
+
+    def _setup(self, cfg, device, dtype, tp_rank, tp_size, keep_host):
+        self.cfg, self.device, self.dtype = cfg, device, dtype
+        self.tp_rank, self.tp_size = tp_rank, tp_size
+        self.host = {} if keep_host else None
+        self.layers, self.nbytes = [], 0
+        if cfg.n_heads % tp_size:
+            raise ValueError("tensor-parallel size must divide the head counts")
         compute_kv_shard(cfg.n_kv_heads, cfg.head_dim, tp_rank, tp_size)      # raises on an impossible KV head layout
-        self.layers = []
-        self.nbytes = 0
-        for l in range(cfg.n_layers):
-            L = {}
-            for name, rows, cols, kind in (("attn_q", nq, H, "col"), ("attn_k", nkv, H, "kv"), ("attn_v", nkv, H, "kv"),
-                                           ("attn_output", H, nq, "row"), ("ffn_gate", I, H, "col"),
-                                           ("ffn_up", I, H, "col"), ("ffn_down", H, I, "row")):
-                L[name] = self._qtensor(l, name, rows, cols, kind)
+
+    def _load(self, qtensor, norm):
+        """Fills layers, tok_embd, output, output_norm and the RoPE tables.  qtensor(layer, name, kind) and
+        norm(layer, name) return one tensor of the source under its GGUF name (token_embd, output and output_norm
+        come as layer 0)."""
+        for l in range(self.cfg.n_layers):
+            L = {name: qtensor(l, name, kind) for name, kind in self.GGUF_NAMES.items()}
             for name in ("attn_norm", "ffn_norm"):
-                L[name] = self._norm(l, name)
+                L[name] = norm(l, name)
             self.layers.append(L)
-        self.tok_embd = self._qtensor(0, "token_embd", cfg.vocab, H, "rep")
-        self.output = self._qtensor(0, "output", cfg.vocab, H, "rep")
-        self.output_norm = self._norm(0, "output_norm")
-        cos, sin = rope_tables(cfg)
-        self.rope_cos = torch.from_numpy(cos).to(device).to(dtype)
-        self.rope_sin = torch.from_numpy(sin).to(device).to(dtype)
+        self.tok_embd = qtensor(0, "token_embd", "rep")
+        self.output = qtensor(0, "output", "rep")
+        self.output_norm = norm(0, "output_norm")
+        cos, sin = rope_tables(self.cfg)
+        self.rope_cos = torch.from_numpy(cos).to(self.device).to(self.dtype)
+        self.rope_sin = torch.from_numpy(sin).to(self.device).to(self.dtype)
 
     # ---- real weights -------------------------------------------------------------------------
-    GGUF_NAMES = {"attn_q": "col", "attn_k": "kv", "attn_v": "kv", "attn_output": "row", "ffn_gate": "col",
-                  "ffn_up": "col", "ffn_down": "row"}
-
     @staticmethod
     def config_from_gguf(ar) -> "LlamaConfig":
         """Hyper-parameters from GGUF metadata (`llama.*` keys, as the reference's
@@ -308,27 +318,12 @@ class LlamaWeights:
         cfg = cls.config_from_gguf(ar)
         if max_pos is not None:
             cfg.max_pos = int(max_pos)
-        self.cfg, self.device, self.dtype = cfg, device, dtype
-        self.tp_rank, self.tp_size = tp_rank, tp_size
-        self.host = {} if keep_host else None
-        self.layers, self.nbytes = [], 0
-        if cfg.n_heads % tp_size:
-            raise ValueError("tensor-parallel size must divide the head counts")
-        compute_kv_shard(cfg.n_kv_heads, cfg.head_dim, tp_rank, tp_size)      # raises on an impossible KV head layout
-        for l in range(cfg.n_layers):
-            L = {}
-            for name, kind in cls.GGUF_NAMES.items():
-                L[name] = self._gguf_qtensor(ar, f"blk.{l}.{name}.weight", (l, name), kind)
-            for name in ("attn_norm", "ffn_norm"):
-                L[name] = self._gguf_norm(ar, f"blk.{l}.{name}.weight", (l, name))
-            self.layers.append(L)
-        self.tok_embd = self._gguf_qtensor(ar, "token_embd.weight", (0, "token_embd"), "rep")
-        out_name = "output.weight" if ar.contains_tensor("output.weight") else "token_embd.weight"
-        self.output = self._gguf_qtensor(ar, out_name, (0, "output"), "rep")
-        self.output_norm = self._gguf_norm(ar, "output_norm.weight", (0, "output_norm"))
-        cos, sin = rope_tables(cfg)
-        self.rope_cos = torch.from_numpy(cos).to(device).to(dtype)
-        self.rope_sin = torch.from_numpy(sin).to(device).to(dtype)
+        self._setup(cfg, device, dtype, tp_rank, tp_size, keep_host)
+        top = {"token_embd": "token_embd.weight", "output_norm": "output_norm.weight",
+               "output": "output.weight" if ar.contains_tensor("output.weight") else "token_embd.weight"}
+        src = lambda l, name: top.get(name) or f"blk.{l}.{name}.weight"
+        self._load(lambda l, name, kind: self._gguf_qtensor(ar, src(l, name), (l, name), kind),
+                   lambda l, name: self._put_norm(ar.load_dense(src(l, name), device, dtype), (l, name)))
         return self
 
     UQFF_NAMES = {"attn_q": "self_attn.q_proj", "attn_k": "self_attn.k_proj", "attn_v": "self_attn.v_proj",
@@ -362,60 +357,28 @@ class LlamaWeights:
         rotate-half RoPE pairing, so the fused attention path applies."""
         if ar.config is None:
             raise ValueError("UQFF artifact has no config.json next to its shards")
+        if not ar.contains("model.embed_tokens.weight.format"):
+            raise NotImplementedError("this UQFF artifact keeps dense token embeddings in residual.safetensors (UQFF <= 1.1); "
+                                      "the embedding gather kernel takes ggml block types")
         self = cls.__new__(cls)
         cfg = cls.config_from_hf(ar.config)
         if max_pos is not None:
             cfg.max_pos = int(max_pos)
-        self.cfg, self.device, self.dtype = cfg, device, dtype
-        self.tp_rank, self.tp_size = tp_rank, tp_size
-        self.host = {} if keep_host else None
-        self.layers, self.nbytes = [], 0
-        if cfg.n_heads % tp_size:
-            raise ValueError("tensor-parallel size must divide the head counts")
-        compute_kv_shard(cfg.n_kv_heads, cfg.head_dim, tp_rank, tp_size)      # raises on an impossible KV head layout
-        for l in range(cfg.n_layers):
-            L = {}
-            for name, kind in cls.GGUF_NAMES.items():
-                L[name] = self._uqff_qtensor(ar, f"model.layers.{l}.{cls.UQFF_NAMES[name]}", (l, name), kind)
-            L["attn_norm"] = self._uqff_norm(ar, f"model.layers.{l}.input_layernorm.weight", (l, "attn_norm"))
-            L["ffn_norm"] = self._uqff_norm(ar, f"model.layers.{l}.post_attention_layernorm.weight", (l, "ffn_norm"))
-            self.layers.append(L)
-        if not ar.contains("model.embed_tokens.weight.format"):
-            raise NotImplementedError("this UQFF artifact keeps dense token embeddings in residual.safetensors (UQFF <= 1.1); "
-                                      "the embedding gather kernel takes ggml block types")
-        self.tok_embd = self._uqff_qtensor(ar, "model.embed_tokens", (0, "token_embd"), "rep")
+        self._setup(cfg, device, dtype, tp_rank, tp_size, keep_host)
         tied = bool(ar.config.get("tie_word_embeddings", False)) or not ar.contains("lm_head.weight.format")
-        self.output = self._uqff_qtensor(ar, "model.embed_tokens" if tied else "lm_head", (0, "output"), "rep")
-        self.output_norm = self._uqff_norm(ar, "model.norm.weight", (0, "output_norm"))
-        cos, sin = rope_tables(cfg)
-        self.rope_cos = torch.from_numpy(cos).to(device).to(dtype)
-        self.rope_sin = torch.from_numpy(sin).to(device).to(dtype)
+        top = {"token_embd": "model.embed_tokens", "output": "model.embed_tokens" if tied else "lm_head",
+               "output_norm": "model.norm.weight"}
+        names = dict(cls.UQFF_NAMES, attn_norm="input_layernorm.weight", ffn_norm="post_attention_layernorm.weight")
+        src = lambda l, name: top.get(name) or f"model.layers.{l}.{names[name]}"
+        self._load(lambda l, name, kind: self._uqff_qtensor(ar, src(l, name), (l, name), kind),
+                   lambda l, name: self._put_norm(ar.load_tensor(src(l, name), device, dtype), (l, name)))
         return self
-
-    def _uqff_norm(self, ar, name, key):
-        t = ar.load_tensor(name, self.device, self.dtype).reshape(-1).contiguous()
-        if self.host is not None:
-            self.host[key] = t.float().cpu().numpy()
-        return t
 
     def _uqff_qtensor(self, ar, key_path, key, kind):
         q = ar.load_qtensor(key_path, "cpu")
         rows, cols = q.shape
-        be, bb = BLOCK_ELEMS[q.dtype], BLOCK_BYTES[q.dtype]
-        full = q.data.numpy().reshape(rows, cols // be, bb)
-        full, rows, cols = self._shard(full, rows, cols, be, kind)
-        flat = np.ascontiguousarray(full).reshape(-1)
-        t = torch.from_numpy(np.array(flat)).to(self.device)
-        self.nbytes += t.numel()
-        if self.host is not None:
-            self.host[key] = np.array(flat)
-        return (t, q.dtype, rows, cols)
-
-    def _gguf_norm(self, ar, name, key):
-        t = ar.load_dense(name, self.device, self.dtype).reshape(-1).contiguous()
-        if self.host is not None:
-            self.host[key] = t.float().cpu().numpy()
-        return t
+        blocks = q.data.numpy().reshape(rows, cols // BLOCK_ELEMS[q.dtype], BLOCK_BYTES[q.dtype])
+        return self._upload(blocks, q.dtype, kind, key)
 
     def _gguf_qtensor(self, ar, name, key, kind):
         info = ar.tensor_info(name)
@@ -425,57 +388,63 @@ class LlamaWeights:
         if len(info.shape) != 2:
             raise ValueError(f"GGUF tensor `{name}` must be a matrix, got shape {info.shape}")
         rows, cols = info.shape
-        be, bb = BLOCK_ELEMS[info.dtype], BLOCK_BYTES[info.dtype]
-        full = ar.tensor_data(name).reshape(rows, cols // be, bb)
-        full, rows, cols = self._shard(full, rows, cols, be, kind)
-        flat = np.ascontiguousarray(full).reshape(-1)
-        t = torch.from_numpy(np.array(flat)).to(self.device)
-        self.nbytes += t.numel()
-        if self.host is not None:
-            self.host[key] = np.array(flat)
-        return (t, info.dtype, rows, cols)
+        blocks = ar.tensor_data(name).reshape(rows, cols // BLOCK_ELEMS[info.dtype], BLOCK_BYTES[info.dtype])
+        return self._upload(blocks, info.dtype, kind, key)
 
-    def _shard(self, full, rows, cols, be, kind):
-        """kind: 'col' (rows sharded), 'kv' (rows sharded by KV head, replicated when ranks outnumber KV heads),
-        'row' (K sharded on block boundaries), 'rep' (replicated)."""
+    def _shard(self, rows, cols, be, kind):
+        """This rank's part of a [rows, cols] matrix of `be`-element blocks: (row slice, block-column slice).
+        kind: 'col' (rows sharded), 'kv' (rows sharded by KV head, replicated when ranks outnumber KV heads),
+        'row' (K sharded on block boundaries), 'rep' (replicated).  Sharding rules: REF
+        mistralrs-quant/src/distributed/layers.rs:1167-1294 (column), :695-975 (row), gguf/weight_source.rs:809-818
+        (block-aligned K slices)."""
         r, w = self.tp_rank, self.tp_size
+        nb = cols // be
         if kind == "kv" and w > 1:
             first, n = compute_kv_shard(self.cfg.n_kv_heads, self.cfg.head_dim, r, w)
-            return full[first:first + n], n, cols
+            return slice(first, first + n), slice(0, nb)
         if kind == "col" and w > 1:
             if rows % w:
                 raise ValueError("column-parallel rows do not divide by the tensor-parallel size")
-            return full[r * rows // w:(r + 1) * rows // w], rows // w, cols
+            return slice(r * rows // w, (r + 1) * rows // w), slice(0, nb)
         if kind == "row" and w > 1:
-            nb = cols // be
             if nb % w:
                 raise ValueError("row-parallel K does not split on block boundaries")
-            return full[:, r * nb // w:(r + 1) * nb // w], rows, cols // w
-        return full, rows, cols
+            return slice(0, rows), slice(r * nb // w, (r + 1) * nb // w)
+        return slice(0, rows), slice(0, nb)
+
+    def _upload(self, blocks, ggml_type, kind, key):
+        """ggml blocks [rows, cols / block, block_bytes] -> (device tensor, type, rows, cols) of this rank's shard,
+        counted in nbytes and kept in host[key] under keep_host.  A read-only source (an archive's mapping, which
+        closes with the archive) is copied first."""
+        be = BLOCK_ELEMS[ggml_type]
+        rs, ks = self._shard(blocks.shape[0], blocks.shape[1] * be, be, kind)
+        flat = np.ascontiguousarray(blocks[rs, ks]).reshape(-1)
+        if not flat.flags.writeable:
+            flat = flat.copy()
+        t = torch.from_numpy(flat).to(self.device)
+        self.nbytes += t.numel()
+        if self.host is not None:
+            self.host[key] = flat
+        return (t, ggml_type, rs.stop - rs.start, (ks.stop - ks.start) * be)
+
+    def _put_norm(self, t, key):
+        """a norm vector already in the activation dtype on the device, flattened; host[key] keeps it in f32"""
+        t = t.reshape(-1).contiguous()
+        if self.host is not None:
+            self.host[key] = t.float().cpu().numpy()
+        return t
 
     def _norm(self, layer, name):
         rng = np.random.Generator(np.random.PCG64(tensor_seed(layer, name)))
         w = (1.0 + 0.1 * rng.standard_normal(self.cfg.hidden)).astype(np.float32)
-        t = torch.from_numpy(w).to(self.device).to(self.dtype)
-        if self.host is not None:
-            self.host[(layer, name)] = t.float().cpu().numpy()
-        return t
+        return self._put_norm(torch.from_numpy(w).to(self.device).to(self.dtype), (layer, name))
 
     def _qtensor(self, layer, name, rows, cols, kind):
-        """kind: 'col' (rows sharded), 'row' (K sharded on block boundaries), 'rep' (replicated).
-        Sharding rules: REF mistralrs-quant/src/distributed/layers.rs:1167-1294 (column),
-        :695-975 (row), gguf/weight_source.rs:809-818 (block-aligned K slices)."""
         dt = tensor_type(self.cfg, name, layer)
         be, bb = BLOCK_ELEMS[dt], BLOCK_BYTES[dt]
         if self.fast_synth:
-            w = self.tp_size
-            if kind == "kv" and w > 1:
-                rows = compute_kv_shard(self.cfg.n_kv_heads, self.cfg.head_dim, self.tp_rank, w)[1]
-            elif kind == "col" and w > 1:
-                rows //= w
-            elif kind == "row" and w > 1:
-                assert (cols // be) % w == 0
-                cols //= w
+            rs, ks = self._shard(rows, cols, be, kind)
+            rows, cols = rs.stop - rs.start, (ks.stop - ks.start) * be
             nblocks = rows * cols // be
             gen = torch.Generator(device=self.device).manual_seed(tensor_seed(layer, name) * 64 + self.tp_rank)
             raw = torch.randint(0, 256, (nblocks, bb), dtype=torch.uint8, device=self.device, generator=gen)
@@ -490,13 +459,7 @@ class LlamaWeights:
             self.nbytes += t.numel()
             return (t, dt, rows, cols)
         full = synth_blocks(dt, rows * cols // be, tensor_seed(layer, name), self.cfg.synth_scale_exp).reshape(rows, cols // be, bb)
-        full, rows, cols = self._shard(full, rows, cols, be, kind)
-        full = np.ascontiguousarray(full)
-        t = torch.from_numpy(full.reshape(-1)).to(self.device)
-        self.nbytes += t.numel()
-        if self.host is not None:
-            self.host[(layer, name)] = full.reshape(-1)
-        return (t, dt, rows, cols)
+        return self._upload(full, dt, kind, (layer, name))
 
 
 def runner_split_pages(block_size, batch, n_kv_heads, max_ctx, sm_count=132, min_tokens=64):
@@ -515,48 +478,144 @@ MMVQ_MAX_BATCH = 8       # up to this many rows the linears are GEMVs; above, th
 
 
 def check_runner_args(batch, comm=None, peer_allreduce=None):
-    """ValueError for a decode batch mrs_llama_decode_step rejects: outside 1..256, or tensor parallel above 8 rows."""
+    """ValueError for a decode batch the decode steps reject: outside 1..256, or tensor parallel above 8 rows."""
     if isinstance(batch, bool) or not isinstance(batch, (int, np.integer)) or not 1 <= batch <= MAX_DECODE_BATCH:
-        raise ValueError(f"LlamaRunner: batch must be an int in 1..{MAX_DECODE_BATCH}, got {batch!r}")
+        raise ValueError(f"decode batch must be an int in 1..{MAX_DECODE_BATCH}, got {batch!r}")
     if batch > MMVQ_MAX_BATCH and (comm is not None or peer_allreduce is not None):
         raise ValueError(f"LlamaRunner: tensor parallelism (comm / peer_allreduce) runs batches of up to {MMVQ_MAX_BATCH}, "
                          f"got {batch}")
 
 
-class LlamaRunner:
+def _point(struct, *tensor_dicts):
+    """struct.<name> <- the device address of every tensor (None: NULL) in the dicts"""
+    for d in tensor_dicts:
+        for n, t in d.items():
+            setattr(struct, n, None if t is None else t.data_ptr())
+
+
+class PagedDecodeRunner:
+    """The paged-KV side of a decode runner over `weights` (LlamaRunner, GptqRunner): block pool, per-sequence block
+    tables and context lengths, the split-KV plan, the index metadata and its advance (mrs_decode_advance_multi), the
+    host-side bound on the context, and CUDA-graph capture / replay of step().  A subclass checks its arguments first
+    (check_runner_args), then adds its KV caches, scratch (`buf`) and step struct (`step_struct`) and implements
+    forward()."""
+    KEEP_GRAPH = False     # capture with keep_graph=True, so the kernel nodes can be counted afterwards
+
+    def __init__(self, weights, batch, max_ctx, split_pages):
+        """split_pages: split-KV chunk in pages, 0 for the unsplit plan (also taken when each sequence fits one chunk)"""
+        cfg, dev = weights.cfg, weights.device
+        self.w, self.cfg, self.dev, self.dt, self.B = weights, cfg, dev, weights.dtype, int(batch)
+        self.max_blocks = -(-max_ctx // cfg.block_size)
+        self.pool = kv_index.BlockPool(self.B * self.max_blocks + 1)
+        self.tables = [self.pool.get_new_blocks(self.max_blocks) for _ in range(self.B)]
+        self.block_tables = torch.tensor(self.tables, dtype=torch.int32, device=dev)
+        self.context_lens = torch.zeros(self.B, dtype=torch.int32, device=dev)
+        self.error_flag = torch.zeros(1, dtype=torch.int32, device=dev)   # bit 0: a sequence ran out of context
+        self.max_ctx = min(self.max_blocks * cfg.block_size, cfg.max_pos)
+        self.steps_taken = 0              # host-side count of advances since reset() (graph replays via replay())
+        self.split_pages = split_pages
+        self.padded_tiles = self.B * -(-self.max_blocks // split_pages) if split_pages else self.B
+        if self.padded_tiles <= self.B:        # a single chunk per request: unsplit plan
+            self.split_pages, self.padded_tiles = 0, self.B
+        self.meta = self.decode_meta(1)
+        self.graph = None
+
+    def decode_meta(self, q):
+        """the index metadata of a step that feeds q rows per sequence, over this runner's tables and plan"""
+        B, R, P = self.B, self.B * q, self.padded_tiles
+        z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=self.dev)
+        return dict(token_ids=z(R), positions=z(R), slot_mapping=z(R, d=torch.int64), kv_indptr=z(B + 1),
+                    kv_indices=z(B * self.max_blocks), kv_last_page_len=z(B), request_indices=z(P), kv_tile_indices=z(P),
+                    o_indptr=z(B + 1), kv_chunk_size=z(1), block_valid_mask=z(P, d=torch.uint8))
+
+    def _stream(self):
+        return ctypes.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+
+    def _advance(self, meta, q):
+        """enqueue the advance of every sequence by q rows, writing `meta` (see decode_meta)"""
+        rc = lib().mrs_decode_advance_multi(
+            ctypes.c_void_p(self.block_tables.data_ptr()), ctypes.c_int(self.max_blocks),
+            ctypes.c_void_p(self.context_lens.data_ptr()), ctypes.c_int(self.B), ctypes.c_int(self.cfg.block_size),
+            ctypes.c_int(self.split_pages), ctypes.c_int(self.padded_tiles),
+            *[ctypes.c_void_p(meta[n].data_ptr()) for n in ("positions", "slot_mapping", "kv_indptr", "kv_indices",
+                                                            "kv_last_page_len", "request_indices", "kv_tile_indices",
+                                                            "o_indptr", "kv_chunk_size", "block_valid_mask")],
+            ctypes.c_int(self.cfg.max_pos), ctypes.c_void_p(self.error_flag.data_ptr()), ctypes.c_int(q), self._stream())
+        if rc != 0:
+            raise RuntimeError(f"mrs_decode_advance_multi failed: cudaError {rc}")
+
+    def advance(self):
+        self._advance(self.meta, 1)
+        self.steps_taken += 1
+
+    def step(self):
+        """advance the KV metadata for the token in `token_ids`, run the stack, argmax -> token_ids."""
+        if self.steps_taken >= self.max_ctx and not torch.cuda.is_current_stream_capturing():
+            raise RuntimeError(f"{type(self).__name__}: context exhausted ({self.max_ctx} tokens: block table / RoPE table)")
+        self.advance()
+        self.forward()
+
+    def reset(self, context_len=0):
+        """context_len: one length for every sequence, or a sequence of B lengths (sequences at different positions,
+        e.g. prompts of different lengths prefilled into their own tables).  The host-side bound on further steps
+        follows the longest."""
+        if isinstance(context_len, (int, np.integer)):
+            self.context_lens.fill_(int(context_len))
+            longest = int(context_len)
+        else:
+            lens = [int(c) for c in context_len]
+            if len(lens) != self.B or min(lens) < 0:
+                raise ValueError(f"{type(self).__name__}.reset: need {self.B} lengths >= 0, got {lens}")
+            self.context_lens.copy_(torch.tensor(lens, dtype=torch.int32))
+            longest = max(lens)
+        self.error_flag.zero_()
+        self.steps_taken = longest
+
+    def replay(self):
+        """one captured decode step; raises before a sequence would run past the allocated context
+        (the kernels freeze such a sequence and set error_flag, but a caller should never get there)"""
+        if self.steps_taken >= self.max_ctx:
+            raise RuntimeError(f"{type(self).__name__}: context exhausted ({self.max_ctx} tokens: block table / RoPE table)")
+        self.steps_taken += 1
+        self.graph.replay()
+
+    def check_overflow(self):
+        if int(self.error_flag.item()) & 1:
+            raise RuntimeError(f"{type(self).__name__}: a sequence ran past its allocated context (KV write skipped)")
+
+    def capture(self):
+        self.step(); self.reset()  # warm-up outside capture (module load, attributes)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph(keep_graph=self.KEEP_GRAPH)
+        with torch.cuda.graph(g):
+            self.step()
+        self.reset()
+        self.graph = g
+        return g
+
+    def set_tokens(self, ids):
+        self.meta["token_ids"].copy_(torch.as_tensor(ids, dtype=torch.int32, device=self.dev))
+
+    def logits(self):
+        return self.buf["logits"]
+
+
+class LlamaRunner(PagedDecodeRunner):
     """Owns KV cache + scratch + per-step metadata for a batch of sequences and drives
-    mrs_llama_decode_step / mrs_decode_advance (eagerly or as a captured CUDA graph).
+    mrs_llama_decode_step / mrs_decode_advance_multi (eagerly or as a captured CUDA graph).
     batch 1..8 runs the GEMV chain, 9..256 the dequant-GEMM chain (prefill numerics; see mrs_b200_model.h)."""
+    KEEP_GRAPH = True
 
     def __init__(self, weights: LlamaWeights, batch=1, max_ctx=512, pdl=False, sm_count=132, comm=None,
                  fused_attention=True, split_policy="sm_fill", split_min_tokens=64, peer_allreduce=None):
         check_runner_args(batch, comm, peer_allreduce)
-        batch = int(batch)
-        cfg, dev, dt = weights.cfg, weights.device, weights.dtype
-        self.w, self.cfg, self.dev, self.dt, self.B = weights, cfg, dev, dt, batch
-        tp = weights.tp_size
-        self.n_heads, self.n_kv = cfg.n_heads // tp, max(1, cfg.n_kv_heads // tp)   # (KV heads are replicated when tp > kv heads)
-        bs = cfg.block_size
-        self.max_blocks = -(-max_ctx // bs)
-        nb = batch * self.max_blocks + 1
-        self.pool = kv_index.BlockPool(nb)
-        self.tables = [self.pool.get_new_blocks(self.max_blocks) for _ in range(batch)]
-        self.block_tables = torch.tensor(self.tables, dtype=torch.int32, device=dev)
-        self.context_lens = torch.zeros(batch, dtype=torch.int32, device=dev)
-        self.error_flag = torch.zeros(1, dtype=torch.int32, device=dev)   # bit 0: a sequence ran out of context
-        self.max_ctx = min(self.max_blocks * bs, cfg.max_pos)
-        self.steps_taken = 0              # host-side count of advances since reset() (graph replays via replay())
-        self.split_pages = (kv_index.decode_split_pages(bs, batch, self.n_kv, max_ctx, sm_count=sm_count)
-                            if split_policy == "reference" else
-                            runner_split_pages(bs, batch, self.n_kv, max_ctx, sm_count, split_min_tokens))
-        self.padded_tiles = batch * -(-self.max_blocks // self.split_pages)
-        if self.padded_tiles <= batch:        # a single chunk per request: unsplit plan
-            self.split_pages, self.padded_tiles = 0, batch
-        z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=dev)
-        self.meta = dict(token_ids=z(batch), positions=z(batch), slot_mapping=z(batch, d=torch.int64),
-                         kv_indptr=z(batch + 1), kv_indices=z(batch * self.max_blocks), kv_last_page_len=z(batch),
-                         request_indices=z(self.padded_tiles), kv_tile_indices=z(self.padded_tiles),
-                         o_indptr=z(batch + 1), kv_chunk_size=z(1), block_valid_mask=z(self.padded_tiles, d=torch.uint8))
+        cfg, tp, bs = weights.cfg, weights.tp_size, weights.cfg.block_size
+        n_kv = max(1, cfg.n_kv_heads // tp)   # (KV heads are replicated when tp > kv heads)
+        super().__init__(weights, batch, max_ctx,
+                         kv_index.decode_split_pages(bs, batch, n_kv, max_ctx, sm_count=sm_count) if split_policy == "reference"
+                         else runner_split_pages(bs, batch, n_kv, max_ctx, sm_count, split_min_tokens))
+        batch, dev, dt, nb = self.B, self.dev, self.dt, self.B * self.max_blocks + 1
+        self.n_heads, self.n_kv = cfg.n_heads // tp, n_kv
         a = lambda *s: torch.zeros(*s, dtype=dt, device=dev)
         H = cfg.hidden
         self.buf = dict(x=a(batch, H), x2=a(batch, H), q=a(batch, self.n_heads * cfg.head_dim),
@@ -573,10 +632,7 @@ class LlamaRunner:
         self._layers, s = _model_step(weights, self.k_cache, self.v_cache, pdl, self.n_heads, self.n_kv)
         s.batch, s.padded_tiles, s.max_blocks_per_seq = batch, self.padded_tiles, self.max_blocks
         s.fused_attention = int(fused_attention)
-        for n, t in self.meta.items():
-            setattr(s, n, t.data_ptr())
-        for n, t in self.buf.items():
-            setattr(s, n, t.data_ptr())
+        _point(s, self.meta, self.buf)
         self._ar_cb, self._peer = None, peer_allreduce
         if peer_allreduce is not None:     # in-graph peer-memory sum (takes precedence over the callback)
             s.tp = peer_allreduce.pointer()
@@ -584,80 +640,11 @@ class LlamaRunner:
             self._ar_cb = _AR_FN(comm)
             s.all_reduce = self._ar_cb
         self.step_struct = s
-        self.graph = None
-
-    # ---- eager pieces -------------------------------------------------------------------
-    def _stream(self):
-        return ctypes.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
-
-    def advance(self):
-        m = self.meta
-        rc = lib().mrs_decode_advance(ctypes.c_void_p(self.block_tables.data_ptr()), ctypes.c_int(self.max_blocks),
-                                      ctypes.c_void_p(self.context_lens.data_ptr()), ctypes.c_int(self.B),
-                                      ctypes.c_int(self.cfg.block_size), ctypes.c_int(self.split_pages),
-                                      ctypes.c_int(self.padded_tiles), *[ctypes.c_void_p(m[k].data_ptr()) for k in
-                                      ("positions", "slot_mapping", "kv_indptr", "kv_indices", "kv_last_page_len",
-                                       "request_indices", "kv_tile_indices", "o_indptr", "kv_chunk_size",
-                                       "block_valid_mask")], ctypes.c_int(self.cfg.max_pos),
-                                      ctypes.c_void_p(self.error_flag.data_ptr()), self._stream())
-        assert rc == 0, rc
-        self.steps_taken += 1
 
     def forward(self):
         rc = lib().mrs_llama_decode_step(ctypes.byref(self.step_struct), self._stream())
         if rc != 0:
             raise RuntimeError(f"mrs_llama_decode_step failed: cudaError {rc}")
-
-    def step(self):
-        """advance the KV metadata for the token in `token_ids`, run the stack, argmax -> token_ids."""
-        if self.steps_taken >= self.max_ctx and not torch.cuda.is_current_stream_capturing():
-            raise RuntimeError(f"LlamaRunner: context exhausted ({self.max_ctx} tokens: block table / RoPE table)")
-        self.advance()
-        self.forward()
-
-    def reset(self, context_len=0):
-        """context_len: one length for every sequence, or a sequence of B lengths (sequences at different positions,
-        e.g. prompts of different lengths prefilled into their own tables).  The host-side bound on further steps
-        follows the longest."""
-        if isinstance(context_len, (int, np.integer)):
-            self.context_lens.fill_(int(context_len))
-            longest = int(context_len)
-        else:
-            lens = [int(c) for c in context_len]
-            if len(lens) != self.B or min(lens) < 0:
-                raise ValueError(f"LlamaRunner.reset: need {self.B} lengths >= 0, got {lens}")
-            self.context_lens.copy_(torch.tensor(lens, dtype=torch.int32))
-            longest = max(lens)
-        self.error_flag.zero_()
-        self.steps_taken = longest
-
-    def replay(self):
-        """one captured decode step; raises before a sequence would run past the allocated context
-        (the kernels freeze such a sequence and set error_flag, but a caller should never get there)"""
-        if self.steps_taken >= self.max_ctx:
-            raise RuntimeError(f"LlamaRunner: context exhausted ({self.max_ctx} tokens: block table / RoPE table)")
-        self.steps_taken += 1
-        self.graph.replay()
-
-    def check_overflow(self):
-        if int(self.error_flag.item()) & 1:
-            raise RuntimeError("LlamaRunner: a sequence ran past its allocated context (KV write skipped)")
-
-    def capture(self):
-        self.step(); self.reset()  # warm-up outside capture (module load, attributes)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph(keep_graph=True)   # keep_graph: the kernel nodes can be counted afterwards
-        with torch.cuda.graph(g):
-            self.step()
-        self.reset()
-        self.graph = g
-        return g
-
-    def set_tokens(self, ids):
-        self.meta["token_ids"].copy_(torch.as_tensor(ids, dtype=torch.int32, device=self.dev))
-
-    def logits(self):
-        return self.buf["logits"]
 
 
 MAX_PREFILL_SEQS = 256   # sequences per prompt step (mrs_llama_prefill_step)
@@ -908,8 +895,7 @@ class LlamaPrefill:
         p.paged, p.lm_rows, p.block_table_stride, p.num_blocks = int(paged), int(lm_rows), stride, self.num_cache_blocks
         p.slot_mapping, p.token_ids, p.positions, p.cu_seqlens_q, p.cu_seqlens_k, p.last_rows = (ptr(k) for k in range(6))
         p.block_tables = ptr(7) if paged else None
-        for name, t in self.buf.items():
-            setattr(p, name, None if t is None else t.data_ptr())
+        _point(p, self.buf)
         logits = None
         if lm_rows:
             logits = torch.empty(n if lm_rows == 1 else T, cfg.vocab, dtype=self.dt, device=dev)
@@ -974,10 +960,7 @@ class LlamaVerifier:
         R = B * q
         self.r, self.k, self.q, self.B, self.dev, self.vocab = runner, k, q, B, dev, cfg.vocab
         z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=dev)
-        self.meta = dict(token_ids=z(R), positions=z(R), slot_mapping=z(R, d=torch.int64),
-                         kv_indptr=z(B + 1), kv_indices=z(B * r.max_blocks), kv_last_page_len=z(B),
-                         request_indices=z(r.padded_tiles), kv_tile_indices=z(r.padded_tiles),
-                         o_indptr=z(B + 1), kv_chunk_size=z(1), block_valid_mask=z(r.padded_tiles, d=torch.uint8))
+        self.meta = r.decode_meta(q)
         a = lambda *s: torch.zeros(*s, dtype=dt, device=dev)
         H, D, n_heads, n_kv = cfg.hidden, cfg.head_dim, r.n_heads, r.n_kv
         nsub = -(-(n_heads // n_kv) * q // 16)
@@ -993,10 +976,7 @@ class LlamaVerifier:
         self._drafts_h = torch.zeros(B, k, dtype=torch.int32).pin_memory()
         self._h2d_done = torch.cuda.Event()
         s = _Step.from_buffer_copy(runner.step_struct)   # weights, caches, shapes, pdl: the runner's
-        for n, t in self.meta.items():
-            setattr(s, n, t.data_ptr())
-        for n, t in self.buf.items():
-            setattr(s, n, t.data_ptr())
+        _point(s, self.meta, self.buf)
         self.step_struct = s
         self.graph = None
 
@@ -1018,18 +998,6 @@ class LlamaVerifier:
         self.meta["token_ids"].view(self.B, self.q)[:, 1:].copy_(t, non_blocking=True)
         self._h2d_done.record()
 
-    def advance(self):
-        r, m = self.r, self.meta
-        rc = lib().mrs_decode_advance_multi(
-            ctypes.c_void_p(r.block_tables.data_ptr()), ctypes.c_int(r.max_blocks), ctypes.c_void_p(r.context_lens.data_ptr()),
-            ctypes.c_int(self.B), ctypes.c_int(r.cfg.block_size), ctypes.c_int(r.split_pages), ctypes.c_int(r.padded_tiles),
-            *[ctypes.c_void_p(m[n].data_ptr()) for n in ("positions", "slot_mapping", "kv_indptr", "kv_indices",
-                                                         "kv_last_page_len", "request_indices", "kv_tile_indices",
-                                                         "o_indptr", "kv_chunk_size", "block_valid_mask")],
-            ctypes.c_int(r.cfg.max_pos), ctypes.c_void_p(r.error_flag.data_ptr()), ctypes.c_int(self.q), r._stream())
-        if rc != 0:
-            raise RuntimeError(f"mrs_decode_advance_multi failed: cudaError {rc}")
-
     def forward(self):
         res = self.results
         rc = lib().mrs_llama_verify_step(ctypes.byref(self.step_struct), ctypes.c_int(self.q),
@@ -1040,7 +1008,7 @@ class LlamaVerifier:
 
     def step(self):
         """one verify step on the current anchors and drafts (eager): advance by q rows, verify, accept."""
-        self.advance()
+        self.r._advance(self.meta, self.q)
         self.forward()
 
     def capture(self):

@@ -1,7 +1,7 @@
-"""Print the kernel launches of the Llama decode, verify and prompt steps, one line per kernel node of a captured CUDA
-graph, in dependency order: kernel name, grid, block, dynamic shared memory, cluster dimensions (when set) and whether
-the incoming edge is programmatic (a PDL link).  Two builds of libmrs_b200.so that print the same lines enqueue the
-same launches, so a refactor of host-side launch code can be checked against its parent:
+"""Print the kernel launches of the Llama decode, verify and prompt steps and of the GPTQ decode step, one line per kernel
+node of a captured CUDA graph, in dependency order: kernel name, grid, block, dynamic shared memory, cluster dimensions
+(when set) and whether the incoming edge is programmatic (a PDL link).  Two builds of libmrs_b200.so that print the same
+lines enqueue the same launches, so a refactor of host-side launch code can be checked against its parent:
 
     python scripts/launch_sequence.py > new.txt
     python scripts/launch_sequence.py --lib /path/to/parent/libmrs_b200.so > old.txt
@@ -156,6 +156,18 @@ def main():
         run.step()
         report(name, capture(run.step))
         del run
+
+    # ---- GPTQ decode steps: advance + W4A16 layer stack + dense lm_head + argmax, split plan (HND) and unsplit (vLLM)
+    from mistralrs_b200 import gptq_model as G
+    gw = G.GptqWeights(G.GptqConfig.tiny_test(max_pos=4096), dev)
+    for layout in ("hnd", "vllm"):
+        for B in (4, 32):
+            run = G.GptqRunner(gw, batch=B, max_ctx=400, cache_layout=layout)
+            run.set_tokens([(5 * b + 3) % 500 for b in range(B)])
+            run.step()
+            report(f"gptq decode {layout} B={B}", capture(run.step))
+            del run
+    del gw
 
     # ---- verify steps: advance_multi + layer stack + lm_head + argmax + acceptance
     for B, q in ((1, 4), (2, 4), (16, 4), (33, 8)):

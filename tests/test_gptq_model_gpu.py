@@ -42,6 +42,26 @@ def test_gptq_decode_matches_oracle(cuda, layout):
     print(f"gptq decode stack ({layout}): worst logit error {worst:.2e} of the logit scale")
 
 
+@pytest.mark.parametrize("layout", ["hnd", "vllm"])
+def test_gptq_context_guard_and_per_sequence_reset(cuda, layout):
+    w = G.GptqWeights(G.GptqConfig.tiny_test(), cuda)
+    run = G.GptqRunner(w, batch=2, max_ctx=32, cache_layout=layout)
+    assert run.max_ctx == 32
+    with pytest.raises(ValueError):
+        run.reset([1, 2, 3])
+    run.set_tokens([1, 2])
+    run.reset([30, 31])                      # sequences at different positions; the bound follows the longer one
+    assert run.steps_taken == 31
+    run.step()                               # the longer sequence writes the last row of its table
+    torch.cuda.synchronize()
+    assert run.meta["positions"].tolist() == [30, 31]
+    assert run.context_lens.tolist() == [31, 32]
+    run.check_overflow()
+    with pytest.raises(RuntimeError, match="context exhausted"):
+        run.step()                           # raised on the host, before anything is enqueued
+    assert run.context_lens.tolist() == [31, 32]
+
+
 def test_gptq_graph_replay_matches_eager(cuda):
     cfg = G.GptqConfig.tiny_test()
     w = G.GptqWeights(cfg, cuda)
