@@ -251,8 +251,34 @@ typedef struct {
  * and waits for the upstream grid before touching its inputs/outputs, so each W4A16 GEMM streams weights while the
  * small kernel before it still runs). */
 int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream);
+/* Batched prompt prefill of a GPTQ / AWQ model: mrs_llama_prefill_step's contract over the int4 layer stack.  `s` gives
+ * weights, norms, per-layer caches (in s->cache_layout), dims, activation dtype, group size, RoPE tables and rope_neox;
+ * its per-step decode metadata and scratch are not read, and skip_mask bit 2 turns the PDL chain off.  `p` is the plan
+ * of mrs_llama_prefill_step, with one difference: p->q is the [T, n_heads*head_dim + 2*n_kv_heads*head_dim] q||k||v
+ * buffer of the concatenated wqkv GEMM, and p->k / p->v / p->gate_up / p->q8_scratch are not read.  Launches:
+ *   dense embedding gather over the T rows -> RMSNorm;
+ *   per layer: qkv W4A16 GEMM -> RoPE at `positions`, strided over qkv -> attention (HND cache, paged 0:
+ *   mrs_prefill_attention, then reshape_and_cache_flashinfer; paged 1: the scatter, then mrs_prefill_attention_paged;
+ *   vLLM layout: mrs_prefill_attention, then reshape_and_cache) -> o GEMM -> add + RMSNorm -> gate||up GEMM with the GLU
+ *   epilogue -> down GEMM -> add + RMSNorm with the next layer's norm (the final norm after the last layer);
+ *   lm_rows 1: the last rows gathered into h_last, the dense lm_head on those n rows, mrs_argmax into out_token, then
+ *   the commit when dest_rows is set; lm_rows 2: the dense lm_head over all T rows.
+ * Every GEMM runs over whole K (`pdl` bit 1 below), so a sequence's K/V rows and logits do not depend on the other
+ * sequences of the call.  The GEMMs and norms are links of a PDL chain.  Not graph-capturable in general.
+ * cudaErrorInvalidValue, before any launch, for: n outside 1..256; T < n; a NULL required pointer (s->layers, the plan
+ * arrays, x / x2 / h / q / attn_out / act; block_tables, with block_table_stride and num_blocks >= 1, when paged;
+ * last_rows, h_last, logits, out_token and argmax_scratch when lm_rows == 1; logits when lm_rows == 2;
+ * runner_token_ids and runner_context_lens when dest_rows is set); lm_rows outside 0..2; dest_rows set while
+ * lm_rows != 1; paged outside 0..1, or paged 1 with the vLLM layout (the paged prompt kernel reads HND pages); an
+ * activation dtype other than f16 / bf16; hidden % 8 != 0. */
+int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama_prefill *p, void *stream);
 /* The chain's links (not reference ABI): mrs_w4a16_gemm / mrs_dense_linear / add_rms_norm / fused_split_glu with a
- * `pdl` flag.  pdl != 0 requires that the launch before it on `stream` is also a link (or a plain kernel). */
+ * `pdl` flag.  pdl bit 0 (value 1) makes the launch a link: it requires that the launch before it on `stream` is also a
+ * link (or a plain kernel).  For mrs_w4a16_gemm_pdl and mrs_dense_linear_pdl, bit 1 (value 2) never splits K over a
+ * cluster, so row r of Y does not depend on M (without it, token tiles of up to 64 rows may split K, which sums the
+ * partials in another order).  For mrs_w4a16_gemm_pdl only, bit 2 (value 4) is the GLU epilogue: w_tiles is gate||up
+ * concatenated along N (N = 2I, I % 8 == 0), and y [M, I] = T(silu(T(X gate^T))) * T(X up^T) is written (with bit 1
+ * set, bit-identical to the plain whole-K GEMM followed by fused_split_glu); the [M, 2I] product is never stored.  Other bits are invalid. */
 int32_t mrs_w4a16_gemm_pdl(const void *x, const void *w_tiles, const void *scales, const int32_t *qzeros, void *y,
                            int32_t M, int32_t K, int32_t N, int32_t group, int32_t dtype, int32_t scale_perm,
                            int32_t pdl, void *stream);

@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "dequant.cuh"
 #include "mrs_b200_model.h"
+#include "prompt_step.cuh"
 
 
 extern "C" int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, const void *w1, const void *w2,
@@ -36,6 +37,10 @@ extern "C" void reshape_and_cache_flashinfer(void *key, void *value, void *key_c
                                              int32_t head_size, int32_t block_size, int32_t key_stride,
                                              int32_t value_stride, float k_scale, float v_scale, uint32_t dtype,
                                              uint32_t cache_dtype, cudaStream_t stream);
+extern "C" void reshape_and_cache(void *key, void *value, void *key_cache, void *value_cache, int64_t *slot_mapping,
+                                  int32_t num_tokens, int32_t num_heads, int32_t head_size, int32_t block_size, int32_t x,
+                                  int32_t key_stride, int32_t value_stride, cudaStream_t stream, uint32_t dtype,
+                                  uint32_t cache_dtype, float *k_scale, float *v_scale);
 extern "C" int32_t mrs_paged_decode_fused(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
                                           const void *rope_cos, const void *rope_sin, const int32_t *positions,
                                           const int64_t *slot_mapping, const int32_t *kv_indptr,
@@ -381,6 +386,46 @@ __global__ void prefill_commit_kernel(const int32_t *__restrict__ out_token, con
   const int r = dest_rows[i];
   token_ids[r] = out_token[i];
   context_lens[r] = cu_k[i + 1] - cu_k[i];
+}
+
+// ---- the prompt-step parts shared with the GPTQ prompt step (prompt_step.cuh)
+int32_t prompt_attention(const mrs_llama_prefill *p, const PromptAttnModel &m, void *q, void *k, void *v, int64_t q_stride,
+                         int64_t kv_stride, void *k_cache, void *v_cache, bool vllm_cache, void *stream) {
+  const int n = p->n_seqs, T = p->total_tokens, dt = m.act_dtype, nq = m.n_heads * m.head_dim;
+  cudaStream_t st = (cudaStream_t)stream;
+  rotary_embedding_positions(q, k, (void *)m.rope_cos, (void *)m.rope_sin, (void *)p->positions, m.rope_neox, m.head_dim, T,
+                             m.head_dim / 2, 0, m.n_heads, m.n_kv_heads, q_stride, kv_stride, (uint32_t)dt, (int64_t)stream);
+  auto scatter = [&] {
+    if (vllm_cache)
+      reshape_and_cache(k, v, k_cache, v_cache, (int64_t *)p->slot_mapping, T, m.n_kv_heads, m.head_dim, m.block_size, 8,
+                        (int32_t)kv_stride, (int32_t)kv_stride, st, (uint32_t)dt, (uint32_t)dt, nullptr, nullptr);
+    else
+      reshape_and_cache_flashinfer(k, v, k_cache, v_cache, (int64_t *)p->slot_mapping, T, m.n_kv_heads, m.head_dim,
+                                   m.block_size, (int32_t)kv_stride, (int32_t)kv_stride, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
+  };
+  if (!p->paged) {   // every key is new: attend over the fresh rows, then write them to the cache
+    MRS_TRY(mrs_prefill_attention(q, k, v, p->attn_out, p->cu_seqlens_q, n, T, p->max_q_len, m.n_heads, m.n_kv_heads,
+                                  m.head_dim, q_stride, kv_stride, nq, m.sm_scale, 1, -1, 0.f, (uint32_t)dt, stream));
+    scatter();
+    return 0;
+  }
+  if (vllm_cache) return (int32_t)cudaErrorInvalidValue;
+  // the new rows join the cached ones in the cache, then attend over the pages
+  scatter();
+  return mrs_prefill_attention_paged(q, k_cache, v_cache, p->attn_out, p->block_tables, p->block_table_stride, p->cu_seqlens_q,
+                                     p->cu_seqlens_k, n, T, p->max_q_len, p->max_kv_len, p->num_blocks, m.n_heads,
+                                     m.n_kv_heads, m.head_dim, m.block_size, q_stride, nq, m.sm_scale, 1, -1, 0.f, (uint32_t)dt,
+                                     stream);
+}
+
+void prompt_gather_last_rows(const mrs_llama_prefill *p, const void *h, int hidden, void *stream) {
+  last_row_gather_kernel<<<p->n_seqs, 128, 0, (cudaStream_t)stream>>>((const uint4 *)h, p->last_rows, (uint4 *)p->h_last,
+                                                                      hidden / 8);
+}
+
+void prompt_commit(const mrs_llama_prefill *p, void *stream) {
+  prefill_commit_kernel<<<(p->n_seqs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      p->out_token, p->cu_seqlens_k, p->dest_rows, p->runner_token_ids, p->runner_context_lens, p->n_seqs);
 }
 
 }  // namespace mrs
@@ -762,33 +807,18 @@ extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_lla
   }
 
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
-  cudaStream_t st = (cudaStream_t)stream;
   const GemmChain c{s, T, true, stream};
+  const PromptAttnModel am{s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->rope_neox, dt, s->sm_scale, s->rope_cos,
+                           s->rope_sin};
   auto attention = [&](const mrs_llama_layer &L) -> int32_t {
-    rotary_embedding_positions(p->q, p->k, (void *)s->rope_cos, (void *)s->rope_sin, (void *)p->positions, s->rope_neox,
-                               s->head_dim, T, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt,
-                               (int64_t)stream);
-    if (!p->paged) {   // every key is new: attend over the fresh rows, then write them to the cache
-      MRS_TRY(mrs_prefill_attention(p->q, p->k, p->v, p->attn_out, p->cu_seqlens_q, n, T, p->max_q_len, s->n_heads,
-                                    s->n_kv_heads, s->head_dim, nq, nkv, nq, s->sm_scale, 1, -1, 0.f, (uint32_t)dt, stream));
-      reshape_and_cache_flashinfer(p->k, p->v, L.k_cache, L.v_cache, (int64_t *)p->slot_mapping, T, s->n_kv_heads,
-                                   s->head_dim, s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
-      return 0;
-    }
-    // the new rows join the cached ones in the cache, then attend over the pages
-    reshape_and_cache_flashinfer(p->k, p->v, L.k_cache, L.v_cache, (int64_t *)p->slot_mapping, T, s->n_kv_heads,
-                                 s->head_dim, s->block_size, nkv, nkv, 1.f, 1.f, (uint32_t)dt, (uint32_t)dt, st);
-    return mrs_prefill_attention_paged(p->q, L.k_cache, L.v_cache, p->attn_out, p->block_tables, p->block_table_stride,
-                                       p->cu_seqlens_q, p->cu_seqlens_k, n, T, p->max_q_len, p->max_kv_len, p->num_blocks,
-                                       s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, nq, nq, s->sm_scale, 1, -1,
-                                       0.f, (uint32_t)dt, stream);
+    return prompt_attention(p, am, p->q, p->k, p->v, nq, nkv, L.k_cache, L.v_cache, false, stream);
   };
   MRS_TRY(gemm_layer_chain(c, {p->token_ids, p->x, p->x2, p->h, p->q, p->k, p->v, p->attn_out, p->act, p->gate_up}, true,
                            attention));
   if (p->lm_rows == 2) {
     MRS_TRY(c.single(s->lm_head, s->vocab, p->logits, p->h, H));
   } else if (p->lm_rows == 1) {
-    last_row_gather_kernel<<<n, 128, 0, st>>>((const uint4 *)p->h, p->last_rows, (uint4 *)p->h_last, H / 8);
+    prompt_gather_last_rows(p, p->h, H, stream);
     if (n <= 8) {    // the reference's GgufMatMul at 1..8 rows: Q8_1 activations + MMVQ (fast_mmvq plain)
       const int kpad = (H + 511) / 512 * 512;
       if (dt == MRS_F16) launch_mmvq_gguf_quantize_q8_1_f16(p->h_last, p->q8_scratch, H, kpad, n, stream);
@@ -798,9 +828,7 @@ extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_lla
       MRS_TRY((GemmChain{s, n, true, stream}.single(s->lm_head, s->vocab, p->logits, p->h_last, H)));
     }
     MRS_TRY(mrs_argmax(p->logits, n, s->vocab, dt, p->out_token, p->argmax_scratch, pdl, stream));
-    if (p->dest_rows != nullptr)
-      prefill_commit_kernel<<<(n + 127) / 128, 128, 0, st>>>(p->out_token, p->cu_seqlens_k, p->dest_rows,
-                                                             p->runner_token_ids, p->runner_context_lens, n);
+    if (p->dest_rows != nullptr) prompt_commit(p, stream);
   }
   return (int32_t)cudaGetLastError();
 }

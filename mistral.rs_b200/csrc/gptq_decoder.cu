@@ -8,8 +8,11 @@
 //   [RMSNorm] -> fused QKV GEMM -> RoPE + KV write + paged decode attention (one launch, HND; or the
 //   rotary -> reshape_and_cache -> paged_attention_v1 chain for the vLLM layout) -> o_proj GEMM ->
 //   add + RMSNorm -> gate||up GEMM -> SiLU*mul -> down GEMM -> add + RMSNorm (next layer's norm)
+// mrs_gptq_prefill_step runs the same chain over the packed prompt rows of up to 256 sequences, on whole-K GEMMs with
+// gate||up through the GLU epilogue, and the prompt attention of the Llama prompt step (prompt_step.cuh).
 #include "common.cuh"
 #include "mrs_b200_model.h"
+#include "prompt_step.cuh"
 
 
 extern "C" int32_t mrs_w4a16_gemm(const void *x, const void *w_tiles, const void *scales, const int32_t *qzeros, void *y,
@@ -142,5 +145,69 @@ extern "C" int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream) {
   }
   if (do_lin) MRS_TRY(mrs_dense_linear_pdl(s->h, s->lm_head, s->logits, B, H, s->vocab, dt, pdl, stream));
   MRS_TRY(mrs_argmax(s->logits, B, s->vocab, dt, s->out_token, s->argmax_scratch, 0, stream));
+  return (int32_t)cudaGetLastError();
+}
+
+// the prompt step over the packed rows of n sequences (contract: include/mrs_b200_model.h): the decode step's layer
+// chain over T rows with whole-K GEMMs, gate||up through the GLU epilogue, and the var-len prompt attention
+using namespace mrs;
+
+extern "C" int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama_prefill *p, void *stream) {
+  if (s == nullptr || p == nullptr) return (int32_t)cudaErrorInvalidValue;
+  const int n = p->n_seqs, T = p->total_tokens, dt = s->act_dtype, H = s->hidden;
+  const bool vllm_cache = s->cache_layout != 1;
+  if (n < 1 || n > 256 || T < n || (dt != MRS_F16 && dt != MRS_BF16) || p->lm_rows < 0 || p->lm_rows > 2 ||
+      (p->paged != 0 && p->paged != 1) || (p->paged && vllm_cache) || (p->dest_rows != nullptr && p->lm_rows != 1) ||
+      p->max_q_len < 1 || p->max_kv_len < p->max_q_len || H % 8 != 0)
+    return (int32_t)cudaErrorInvalidValue;
+  if (s->layers == nullptr || p->token_ids == nullptr || p->positions == nullptr ||
+      p->slot_mapping == nullptr || p->cu_seqlens_q == nullptr || p->cu_seqlens_k == nullptr || p->x == nullptr ||
+      p->x2 == nullptr || p->h == nullptr || p->q == nullptr || p->attn_out == nullptr || p->act == nullptr)
+    return (int32_t)cudaErrorInvalidValue;
+  if (p->paged && (p->block_tables == nullptr || p->block_table_stride < 1 || p->num_blocks < 1)) return (int32_t)cudaErrorInvalidValue;
+  if (p->lm_rows == 1 && (p->last_rows == nullptr || p->h_last == nullptr || p->logits == nullptr || p->out_token == nullptr ||
+                          p->argmax_scratch == nullptr))
+    return (int32_t)cudaErrorInvalidValue;
+  if (p->lm_rows == 2 && p->logits == nullptr) return (int32_t)cudaErrorInvalidValue;
+  if (p->dest_rows != nullptr && (p->runner_token_ids == nullptr || p->runner_context_lens == nullptr))
+    return (int32_t)cudaErrorInvalidValue;
+
+  const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim, nqkv = nq + 2 * nkv;
+  // the attention launches are plain kernels, which a PDL link may follow: the GEMMs and norms are links in both layouts
+  const int pdl = (s->skip_mask & 4) ? 0 : 1;
+  // flags | 2: K is never split, so a row's result does not depend on the other rows of the call
+  auto linear = [&](const mrs_w4_weight &w, const void *x, void *y, int flags) -> int32_t {
+    return mrs_w4a16_gemm_pdl(x, w.tiles, w.scales, (const int32_t *)w.qzeros, y, T, w.k, w.n, s->group_size, dt, 0,
+                              pdl | 2 | flags, stream);
+  };
+  auto add_rms = [&](const void *res, const void *w, void *res_dst) {   // res_dst = h + res ; h = norm(res_dst)
+    mrs_add_rms_norm_pdl(p->h, res, w, res_dst, p->h, T, H, s->rms_eps, dt, pdl, stream);
+  };
+  const PromptAttnModel am{s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->rope_neox, dt, s->sm_scale, s->rope_cos,
+                           s->rope_sin};
+
+  mrs::dense_embedding_kernel<<<T, 256, 0, (cudaStream_t)stream>>>((const uint4 *)s->tok_embd, H / 8, p->token_ids, (uint4 *)p->x);
+  if (dt == MRS_F16) mrs_rms_norm_f16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
+  else mrs_rms_norm_bf16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
+  for (int l = 0; l < s->n_layers; l++) {
+    const mrs_gptq_layer &L = s->layers[l];
+    MRS_TRY(linear(L.wqkv, p->h, p->q, 0));                                   // p->q holds the [T, nqkv] qkv rows
+    void *q = p->q, *k = (char *)p->q + (size_t)nq * 2, *v = (char *)p->q + (size_t)(nq + nkv) * 2;
+    MRS_TRY(prompt_attention(p, am, q, k, v, nqkv, nqkv, L.k_cache, L.v_cache, vllm_cache, stream));
+    // the o and down GEMMs write into h, which the add + RMSNorm after them reads as its input and overwrites
+    MRS_TRY(linear(L.wo, p->attn_out, p->h, 0));
+    add_rms(p->x, L.ffn_norm, p->x2);                                        // x2 = o + x ; h = norm(x2)
+    MRS_TRY(linear(L.w_gate_up, p->h, p->act, 4));                           // act = silu(gate) * up
+    MRS_TRY(linear(L.w_down, p->act, p->h, 0));
+    add_rms(p->x2, l + 1 < s->n_layers ? s->layers[l + 1].attn_norm : s->final_norm, p->x);   // x = down + x2 ; h = next norm(x)
+  }
+  if (p->lm_rows == 2) {
+    MRS_TRY(mrs_dense_linear_pdl(p->h, s->lm_head, p->logits, T, H, s->vocab, dt, pdl | 2, stream));
+  } else if (p->lm_rows == 1) {
+    prompt_gather_last_rows(p, p->h, H, stream);
+    MRS_TRY(mrs_dense_linear_pdl(p->h_last, s->lm_head, p->logits, n, H, s->vocab, dt, pdl | 2, stream));
+    MRS_TRY(mrs_argmax(p->logits, n, s->vocab, dt, p->out_token, p->argmax_scratch, pdl, stream));
+    if (p->dest_rows != nullptr) prompt_commit(p, stream);
+  }
   return (int32_t)cudaGetLastError();
 }

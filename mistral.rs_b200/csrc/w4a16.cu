@@ -106,6 +106,18 @@ struct Int4TileSrc {
     }
   }
 };
+// gate||up int4 tiles (N = 2I weight rows: gate 0 .. I-1, up I .. 2I-1) with the GLU epilogue of tc_gemm.cuh: tile z
+// holds gate rows 64 z .. 64 z + 63 in its first 64 rows (warpgroup 0) and the same up rows in its second 64
+// (warpgroup 1); y[M, I] = T(silu(T(gate))) * T(up) is written, the [M, 2I] product never is.
+struct Int4GluSrc : Int4TileSrc {
+  static constexpr int kEpi = 2;
+  void *y;
+  int I;
+  __device__ __forceinline__ int local(int n) const { return (n >> 7) * 64 + (n & 63); }
+  __device__ __forceinline__ bool live(int n) const { return local(n) < I; }
+  __device__ __forceinline__ void *out(int n, int tok) const { return (uint16_t *)y + (size_t)tok * I + local(n); }
+  __device__ __forceinline__ void load(Raw &r, int n, int k) const { Int4TileSrc::load(r, local(n) + ((n >> 6) & 1) * I, k); }
+};
 // dense 16-bit weights: A tiles straight from the TMA
 struct DenseSrc {
   static constexpr bool kTmaA = true;
@@ -160,17 +172,25 @@ __global__ void repack_awq_kernel(const uint32_t *__restrict__ qw, uint32_t *__r
 }
 
 // ---------------------------------------------------------------- host
+// flags: bit 0 a link of a PDL chain, bit 1 never split K, bit 2 (int4 only) the GLU epilogue over gate||up, N = 2I
 static cudaError_t run_wa(int src, const void *x, const void *w, const void *scales, const int32_t *qzeros, void *y, int M,
-                          int K, int N, int group, int dtype, int scale_perm, cudaStream_t st, int pdl = 0) {
+                          int K, int N, int group, int dtype, int scale_perm, cudaStream_t st, int flags = 0) {
+  const bool glu = flags & 4, split_k = !(flags & 2);
+  const int pdl = flags & 1;
+  if ((flags & ~7) || (glu && (src != WA_SRC_INT4 || N % 16 != 0))) return cudaErrorInvalidValue;
   if (M <= 0 || N <= 0) return cudaSuccess;
   if (K % HG_BK != 0 || (dtype != MRS_F16 && dtype != MRS_BF16)) return cudaErrorInvalidValue;
   if (group <= 0) group = K;
   if (src == WA_SRC_INT4 && (group % 32 != 0 || K % group != 0 || N % 8 != 0)) return cudaErrorInvalidValue;
   if (src == WA_SRC_INT4 && qzeros != nullptr && N % 32 != 0) return cudaErrorInvalidValue;
   if (((uintptr_t)x & 15) || ((uintptr_t)w & 15)) return cudaErrorMisalignedAddress;
-  if (src == WA_SRC_DENSE) return hg_run(DenseSrc{}, x, w, y, M, N, K, dtype, pdl, st);
+  if (src == WA_SRC_DENSE) return hg_run(DenseSrc{}, x, w, y, M, N, K, dtype, pdl, st, split_k);
   const Int4TileSrc s = {(const uint8_t *)w, (const uint16_t *)scales, qzeros, N, group, scale_perm, dtype == MRS_BF16};
-  return hg_run(s, x, nullptr, y, M, N, K, dtype, pdl, st);
+  if (glu) {
+    const int I = N / 2;
+    return hg_run(Int4GluSrc{s, y, I}, x, nullptr, nullptr, M, (I + 63) / 64 * HG_BM, K, dtype, pdl, st, split_k);
+  }
+  return hg_run(s, x, nullptr, y, M, N, K, dtype, pdl, st, split_k);
 }
 
 }  // namespace mrs
@@ -192,7 +212,9 @@ extern "C" int32_t mrs_dense_linear(const void *x, const void *w, void *y, int32
   return (int32_t)run_wa(WA_SRC_DENSE, x, w, nullptr, nullptr, y, M, K, N, 0, dtype, 0, (cudaStream_t)stream);
 }
 // the same two as links of a programmatic-dependent-launch chain (decode layer stack): the weight stream starts while
-// the upstream kernel is still running; x is read, and y written, only after it has completed
+// the upstream kernel is still running; x is read, and y written, only after it has completed.  `pdl` bit 0: that
+// link; bit 1: never split K, so a row's result does not depend on M (prompt steps); bit 2 (int4 only): w_tiles is
+// gate||up of N = 2I rows and y [M, I] = T(silu(T(X gate^T))) * T(X up^T), as fused_split_glu after the plain GEMM
 extern "C" int32_t mrs_w4a16_gemm_pdl(const void *x, const void *w_tiles, const void *scales, const int32_t *qzeros, void *y,
                                       int32_t M, int32_t K, int32_t N, int32_t group, int32_t dtype, int32_t scale_perm,
                                       int32_t pdl, void *stream) {

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from . import lib
-from .model import PagedDecodeRunner, _point, check_runner_args, rope_tables, runner_split_pages
+from .model import MAX_PREFILL_SEQS, PagedDecodeRunner, PromptPrefill, _point, check_runner_args, rope_tables, runner_split_pages
 
 
 @dataclass
@@ -146,6 +146,29 @@ class GptqWeights:
         return (tiles, scales, K, N)
 
 
+def _model_step(weights, k_cache, v_cache, cache_layout):
+    """(layer array, mrs_gptq_step) with the model fields only: weights, norms, caches in `cache_layout` ("hnd" or
+    "vllm"), dims, RoPE tables; no per-step metadata or scratch.  The layer array must outlive the struct's use."""
+    cfg = weights.cfg
+    layers = (_Layer * cfg.n_layers)()
+    for l, L in enumerate(weights.layers):
+        for f in ("wqkv", "wo", "w_gate_up", "w_down"):
+            tiles, scales, K, N = L[f]
+            setattr(layers[l], f, _W4(tiles.data_ptr(), scales.data_ptr(), 0, K, N))
+        layers[l].attn_norm, layers[l].ffn_norm = L["attn_norm"].data_ptr(), L["ffn_norm"].data_ptr()
+        layers[l].k_cache, layers[l].v_cache = k_cache[l].data_ptr(), v_cache[l].data_ptr()
+    s = _Step()
+    s.hidden, s.n_layers, s.n_heads, s.n_kv_heads, s.head_dim, s.vocab = (cfg.hidden, cfg.n_layers, cfg.n_heads,
+                                                                          cfg.n_kv_heads, cfg.head_dim, cfg.vocab)
+    s.block_size, s.act_dtype, s.group_size = cfg.block_size, {torch.float16: 0, torch.bfloat16: 1}[weights.dtype], cfg.group_size
+    s.rms_eps, s.sm_scale = cfg.rms_eps, 1.0 / float(np.sqrt(cfg.head_dim))
+    s.rope_neox, s.cache_layout, s.skip_mask = int(cfg.rope_neox), 1 if cache_layout == "hnd" else 0, 0
+    s.layers = ctypes.cast(layers, ctypes.POINTER(_Layer))
+    s.tok_embd, s.lm_head, s.final_norm = weights.tok_embd.data_ptr(), weights.lm_head.data_ptr(), weights.final_norm.data_ptr()
+    s.rope_cos, s.rope_sin = weights.rope_cos.data_ptr(), weights.rope_sin.data_ptr()
+    return layers, s
+
+
 class GptqRunner(PagedDecodeRunner):
     """KV cache + scratch + per-step metadata for a decode batch; drives mrs_gptq_decode_step.  The vLLM cache layout
     runs the unsplit attention plan."""
@@ -172,22 +195,8 @@ class GptqRunner(PagedDecodeRunner):
         else:
             self.k_cache = [a(nb, KVH, D // 8, bs, 8) for _ in range(cfg.n_layers)]
             self.v_cache = [a(nb, KVH, D, bs) for _ in range(cfg.n_layers)]
-        self._layers = (_Layer * cfg.n_layers)()
-        for l, L in enumerate(weights.layers):
-            for f in ("wqkv", "wo", "w_gate_up", "w_down"):
-                tiles, scales, K, N = L[f]
-                setattr(self._layers[l], f, _W4(tiles.data_ptr(), scales.data_ptr(), 0, K, N))
-            self._layers[l].attn_norm, self._layers[l].ffn_norm = L["attn_norm"].data_ptr(), L["ffn_norm"].data_ptr()
-            self._layers[l].k_cache, self._layers[l].v_cache = self.k_cache[l].data_ptr(), self.v_cache[l].data_ptr()
-        s = _Step()
-        s.hidden, s.n_layers, s.n_heads, s.n_kv_heads, s.head_dim, s.vocab = H, cfg.n_layers, NH, KVH, D, cfg.vocab
-        s.block_size, s.act_dtype, s.group_size = bs, {torch.float16: 0, torch.bfloat16: 1}[dt], cfg.group_size
-        s.rms_eps, s.sm_scale = cfg.rms_eps, 1.0 / float(np.sqrt(D))
-        s.rope_neox, s.cache_layout = int(cfg.rope_neox), 1 if cache_layout == "hnd" else 0
-        s.batch, s.padded_tiles, s.max_blocks_per_seq, s.skip_mask = batch, self.padded_tiles, self.max_blocks, 0
-        s.layers = ctypes.cast(self._layers, ctypes.POINTER(_Layer))
-        s.tok_embd, s.lm_head, s.final_norm = weights.tok_embd.data_ptr(), weights.lm_head.data_ptr(), weights.final_norm.data_ptr()
-        s.rope_cos, s.rope_sin = weights.rope_cos.data_ptr(), weights.rope_sin.data_ptr()
+        self._layers, s = _model_step(weights, self.k_cache, self.v_cache, cache_layout)
+        s.batch, s.padded_tiles, s.max_blocks_per_seq = batch, self.padded_tiles, self.max_blocks
         _point(s, self.meta, dict(block_tables=self.block_tables, context_lens=self.context_lens), self.buf)
         self.step_struct = s
 
@@ -195,3 +204,35 @@ class GptqRunner(PagedDecodeRunner):
         rc = lib().mrs_gptq_decode_step(ctypes.byref(self.step_struct), self._stream())
         if rc != 0:
             raise RuntimeError(f"mrs_gptq_decode_step failed: cudaError {rc}")
+
+
+class GptqPrefill(PromptPrefill):
+    """Prompt processing of a GPTQ / AWQ model through `mrs_gptq_prefill_step` (include/mrs_b200_model.h): the packed
+    rows of up to 256 sequences through the int4 layer stack in one pass -- whole-K W4A16 GEMMs (q||k||v, o, gate||up
+    with the SiLU*mul epilogue, down), RoPE, the var-len causal prompt attention and the KV scatter, the dense lm_head on
+    each sequence's last row (or every row) and argmax.  `forward` and `forward_batch` mean what they mean on
+    LlamaPrefill.  With a GptqRunner the K/V go into the runner's caches in its layout, and `forward_batch(slots=...)`
+    followed by `runner.replay()` continues those rows in the decode graph; without one the prefill writes its own HND
+    caches.  Prompts over cached rows (cached > 0) need the HND layout: the paged prompt attention reads HND pages."""
+    STEP = "mrs_gptq_prefill_step"
+
+    def __init__(self, weights: GptqWeights, max_tokens=4096, runner: GptqRunner = None, pdl=True):
+        """max_tokens: new rows per call (all sequences together); the scratch for them is allocated here.
+        pdl: run the GEMMs and norms as a programmatic-dependent-launch chain."""
+        self._init_caches(weights, max_tokens, runner)
+        self.layout = runner.layout if runner is not None else "hnd"
+        cfg, dev, dt = self.cfg, self.dev, self.dt
+        T, H = self.max_tokens, cfg.hidden
+        nq, nkv = cfg.n_heads * cfg.head_dim, cfg.n_kv_heads * cfg.head_dim
+        a = lambda *s: torch.empty(*s, dtype=dt, device=dev)
+        self.buf = dict(x=a(T, H), x2=a(T, H), h=a(T, H), q=a(T, nq + 2 * nkv), attn_out=a(T, nq), act=a(T, cfg.inter),
+                        h_last=a(MAX_PREFILL_SEQS, H),
+                        argmax_scratch=torch.zeros(16 * MAX_PREFILL_SEQS + 16, dtype=torch.uint8, device=dev))
+        self._layers, self.step_struct = _model_step(weights, self.k_cache, self.v_cache, self.layout)
+        self.step_struct.skip_mask = 0 if pdl else 4
+
+    def make_plan(self, ids, cached, tables, lm_rows, slots=None):
+        if self.layout != "hnd" and any(int(c) for c in cached):
+            raise ValueError("GptqPrefill: cached rows need the HND cache layout (the paged prompt attention reads HND "
+                             f"pages), the runner's is {self.layout!r}")
+        return super().make_plan(ids, cached, tables, lm_rows, slots)

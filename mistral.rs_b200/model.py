@@ -684,26 +684,17 @@ def _model_step(weights, k_cache, v_cache, pdl, n_heads, n_kv_heads):
     return layers, s
 
 
-class LlamaPrefill:
-    """Prompt processing through `mrs_llama_prefill_step` (include/mrs_b200_model.h), the reference's prompt forward
-    (`models/llama.rs` Block::forward with seq_len > 1) over the packed rows of one or many sequences:
-    embedding -> per layer RMSNorm, wgmma dequant-GEMMs (grouped QKV, gate|up with the GLU epilogue), RoPE, var-len
-    causal prompt attention over the fresh q/k/v (the reference's flash-attn call, paged_attention.rs:1413-1475) and the
-    KV scatter into the paged HND cache, o_proj, add+RMSNorm, down, add+RMSNorm -> lm_head on each sequence's last row
-    (`extract_logits`) -> argmax.  A sequence with cached rows (prefix-cache hit, or a later chunk of a chunked prompt)
-    has its new K/V scattered first and attends over the cache (`prefill_attention_paged`).
-    `forward` is the one-sequence call; TTFT of BASELINE config 3 is its time on a 4096-token prompt.  `forward_batch`
-    runs up to 256 sequences in one step and can hand them to a decode runner's rows on the device."""
+class PromptPrefill:
+    """The host side of a batched prompt step (`mrs_llama_prefill` plan, include/mrs_b200_model.h), shared by
+    LlamaPrefill and GptqPrefill: argument checks, the plan, its upload, the hand-off to a decode runner's rows, and the
+    KV caches (a decode runner's, or the prefill's own HND caches).  A subclass calls `_init_caches`, then adds its
+    scratch (`buf`), its step struct (`step_struct`) and the name of its C entry (`STEP`)."""
+    STEP = None
 
-    def __init__(self, weights: "LlamaWeights", max_tokens=4096, runner: "LlamaRunner" = None, pdl=True):
-        """max_tokens: new rows per call (all sequences together); the scratch for them is allocated here.
-        runner: write prompts' K/V into this decode runner's paged cache (sequence 0's block table by default), so a
-        generation is prefill -> `runner.reset(T)` -> decode-graph replays, or `forward_batch(slots=...)` ->
-        decode-graph replays."""
-        from . import ops, paged_attn, quant  # noqa: F401  (fail early when the extension is missing)
+    def _init_caches(self, weights, max_tokens, runner):
+        """max_tokens: new rows per call (all sequences together).  runner: write prompts' K/V into this decode runner's
+        paged cache (sequence 0's block table by default), in its layout; without one, the prefill owns HND caches."""
         cfg, dev, dt = weights.cfg, weights.device, weights.dtype
-        if weights.tp_size != 1:
-            raise NotImplementedError("LlamaPrefill runs single-GPU")
         self.w, self.cfg, self.dev, self.dt = weights, cfg, dev, dt
         bs = cfg.block_size
         self.max_tokens = int(max_tokens)
@@ -711,25 +702,16 @@ class LlamaPrefill:
         self.runner = runner
         if runner is not None:
             if runner.max_blocks < self.nblocks:
-                raise ValueError("LlamaPrefill: the runner's block table is shorter than max_tokens")
+                raise ValueError(f"{type(self).__name__}: the runner's block table is shorter than max_tokens")
             self.table, self.k_cache, self.v_cache = list(runner.tables[0]), runner.k_cache, runner.v_cache
         else:
             nb = self.nblocks + 1                                   # block 0 stays the null block
             self.table = list(range(1, self.nblocks + 1))
             self.k_cache = [torch.zeros(nb, cfg.n_kv_heads, bs, cfg.head_dim, dtype=dt, device=dev) for _ in range(cfg.n_layers)]
             self.v_cache = [torch.zeros(nb, cfg.n_kv_heads, bs, cfg.head_dim, dtype=dt, device=dev) for _ in range(cfg.n_layers)]
-        T, H = self.max_tokens, cfg.hidden
-        nq, nkv = cfg.n_heads * cfg.head_dim, cfg.n_kv_heads * cfg.head_dim
-        a = lambda *s: torch.empty(*s, dtype=dt, device=dev)
-        self.buf = dict(x=a(T, H), x2=a(T, H), h=a(T, H), q=a(T, nq), k=a(T, nkv), v=a(T, nkv), attn_out=a(T, nq),
-                        act=a(T, cfg.inter), h_last=a(MAX_PREFILL_SEQS, H),
-                        gate_up=a(2, T, cfg.inter) if T > PREFILL_GROUPED_MAX_ROWS else None,
-                        argmax_scratch=torch.zeros(16 * MAX_PREFILL_SEQS + 16, dtype=torch.uint8, device=dev),
-                        q8_scratch=torch.empty(MMVQ_MAX_BATCH * (-(-H // 512) * 16) * 36, dtype=torch.uint8, device=dev))
+        self.num_cache_blocks = self.k_cache[0].shape[0]
         # first tokens [256], then a copy of the runner's context lengths: one D2H copy returns both
         self._out = torch.zeros(MAX_PREFILL_SEQS + (runner.B if runner is not None else 0), dtype=torch.int32, device=dev)
-        self._layers, self.step_struct = _model_step(weights, self.k_cache, self.v_cache, pdl, cfg.n_heads, cfg.n_kv_heads)
-        self.num_cache_blocks = self.k_cache[0].shape[0]
 
     def forward(self, tokens, all_logits=False, cached=0, table=None):
         """tokens: list[int] (1 < len <= max_tokens), the prompt at positions cached .. cached + T - 1.  Returns logits
@@ -744,15 +726,15 @@ class LlamaPrefill:
         bs = cfg.block_size
         if cached == 0 and table is None:
             if not 1 < T <= min(self.max_tokens, cfg.max_pos):
-                raise ValueError(f"LlamaPrefill.forward: need 1 < tokens <= {min(self.max_tokens, cfg.max_pos)}, got {T}")
+                raise ValueError(f"{type(self).__name__}.forward: need 1 < tokens <= {min(self.max_tokens, cfg.max_pos)}, got {T}")
         else:
             end = cached + T
             tb = self.table if table is None else table
             if cached < 0 or not (1 if cached else 2) <= T <= self.max_tokens:
-                raise ValueError(f"LlamaPrefill.forward: need cached >= 0 and {1 if cached else 2} <= tokens <= "
+                raise ValueError(f"{type(self).__name__}.forward: need cached >= 0 and {1 if cached else 2} <= tokens <= "
                                  f"{self.max_tokens}, got cached={cached}, {T} tokens")
             if end > min(cfg.max_pos, len(tb) * bs):
-                raise ValueError(f"LlamaPrefill.forward: cached + tokens = {end} exceeds max_pos {cfg.max_pos} or the "
+                raise ValueError(f"{type(self).__name__}.forward: cached + tokens = {end} exceeds max_pos {cfg.max_pos} or the "
                                  f"table's {len(tb)} blocks of {bs}")
         table = self.table if table is None else [int(b) for b in table]
         logits = self._step([tokens], [cached], [table], lm_rows=2 if all_logits else 1)
@@ -765,27 +747,27 @@ class LlamaPrefill:
         runner = getattr(self, "runner", None)
         n = len(prompts)
         if not 1 <= n <= MAX_PREFILL_SEQS:
-            raise ValueError(f"LlamaPrefill.forward_batch: need 1..{MAX_PREFILL_SEQS} sequences, got {n}")
+            raise ValueError(f"{type(self).__name__}.forward_batch: need 1..{MAX_PREFILL_SEQS} sequences, got {n}")
         ids = []
         for p in prompts:
             a = p.cpu().numpy() if torch.is_tensor(p) else np.asarray(p)
             a = a.reshape(-1)
             if a.size and (a.dtype.kind not in "iu" or int(a.min()) < 0 or int(a.max()) >= cfg.vocab):
-                raise ValueError(f"LlamaPrefill.forward_batch: token ids must be integers in [0, {cfg.vocab})")
+                raise ValueError(f"{type(self).__name__}.forward_batch: token ids must be integers in [0, {cfg.vocab})")
             ids.append(a.astype(np.int32))
         cached = [0] * n if cached is None else [int(c) for c in cached]
         if len(cached) != n:
-            raise ValueError(f"LlamaPrefill.forward_batch: {len(cached)} cached lengths for {n} sequences")
+            raise ValueError(f"{type(self).__name__}.forward_batch: {len(cached)} cached lengths for {n} sequences")
         if slots is not None:
             if not final:
-                raise ValueError("LlamaPrefill.forward_batch: slots commit first tokens, which a non-final chunk has none of")
+                raise ValueError(f"{type(self).__name__}.forward_batch: slots commit first tokens, which a non-final chunk has none of")
             if runner is None:
-                raise ValueError("LlamaPrefill.forward_batch: slots need a LlamaPrefill built with a runner")
+                raise ValueError(f"{type(self).__name__}.forward_batch: slots need a {type(self).__name__} built with a runner")
             slots = [int(s) for s in slots]
             if len(slots) != n:
-                raise ValueError(f"LlamaPrefill.forward_batch: {len(slots)} slots for {n} sequences")
+                raise ValueError(f"{type(self).__name__}.forward_batch: {len(slots)} slots for {n} sequences")
             if len(set(slots)) != n or min(slots) < 0 or max(slots) >= runner.B:
-                raise ValueError(f"LlamaPrefill.forward_batch: slots must be distinct runner rows in 0..{runner.B - 1}")
+                raise ValueError(f"{type(self).__name__}.forward_batch: slots must be distinct runner rows in 0..{runner.B - 1}")
         if tables is None:
             if slots is not None:
                 tables = [list(runner.tables[s]) for s in slots]
@@ -794,29 +776,29 @@ class LlamaPrefill:
             elif runner is not None and n <= runner.B:
                 tables = [list(runner.tables[i]) for i in range(n)]
             else:
-                raise ValueError("LlamaPrefill.forward_batch: several sequences need their own tables (tables= or a runner)")
+                raise ValueError(f"{type(self).__name__}.forward_batch: several sequences need their own tables (tables= or a runner)")
         tables = [[int(b) for b in t] for t in tables]
         if len(tables) != n:
-            raise ValueError(f"LlamaPrefill.forward_batch: {len(tables)} tables for {n} sequences")
+            raise ValueError(f"{type(self).__name__}.forward_batch: {len(tables)} tables for {n} sequences")
         total = sum(a.size for a in ids)
         if total > self.max_tokens:
-            raise ValueError(f"LlamaPrefill.forward_batch: {total} new rows exceed max_tokens {self.max_tokens}")
+            raise ValueError(f"{type(self).__name__}.forward_batch: {total} new rows exceed max_tokens {self.max_tokens}")
         for i, (a, c, t) in enumerate(zip(ids, cached, tables)):
             if c < 0 or a.size < (1 if c else 2):
-                raise ValueError(f"LlamaPrefill.forward_batch: sequence {i} needs cached >= 0 and at least "
+                raise ValueError(f"{type(self).__name__}.forward_batch: sequence {i} needs cached >= 0 and at least "
                                  f"{1 if c else 2} tokens, got cached={c}, {a.size} tokens")
             cap = len(t) * bs if slots is None else min(len(t), runner.max_blocks) * bs
             if c + a.size > min(cfg.max_pos, cap):
-                raise ValueError(f"LlamaPrefill.forward_batch: sequence {i}: cached + tokens = {c + a.size} exceeds max_pos "
+                raise ValueError(f"{type(self).__name__}.forward_batch: sequence {i}: cached + tokens = {c + a.size} exceeds max_pos "
                                  f"{cfg.max_pos} or its table's {len(t)} blocks of {bs}")
         if n > 1:
             slot_map = np.concatenate([kv_index.slot_mapping(t, bs, c, c + a.size) for a, c, t in zip(ids, cached, tables)])
             if np.unique(slot_map).size != slot_map.size:
-                raise ValueError("LlamaPrefill.forward_batch: two sequences' new rows map to the same cache slot")
+                raise ValueError(f"{type(self).__name__}.forward_batch: two sequences' new rows map to the same cache slot")
         return ids, cached, tables, slots
 
     def forward_batch(self, prompts, cached=None, tables=None, slots=None, final=True):
-        """n sequences' new rows (prompts: n token lists) in one `mrs_llama_prefill_step`.  cached[i] rows of sequence i
+        """n sequences' new rows (prompts: n token lists) in one prompt step (`STEP`).  cached[i] rows of sequence i
         are already in the cache under tables[i] (default 0); tables default to the runner's (rows slots[i], or 0..n-1),
         or the prefill's own table for one sequence.  Returns (last-row logits [n, vocab] on the device, first tokens
         int32 [n] on the host); with final=False (a non-final chunk group) only the KV caches are written and nothing
@@ -842,10 +824,10 @@ class LlamaPrefill:
     def _step(self, ids, cached, tables, lm_rows, slots=None):
         """Build the plan, enqueue the step; returns the logits ([n, vocab] for lm_rows 1, [T, vocab] for 2) or None."""
         p, logits, _plan = self.make_plan(ids, cached, tables, lm_rows, slots)
-        rc = lib().mrs_llama_prefill_step(ctypes.byref(self.step_struct), ctypes.byref(p),
-                                          ctypes.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream))
+        rc = getattr(lib(), self.STEP)(ctypes.byref(self.step_struct), ctypes.byref(p),
+                                       ctypes.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream))
         if rc != 0:
-            raise RuntimeError(f"mrs_llama_prefill_step failed: cudaError {rc}")
+            raise RuntimeError(f"{self.STEP} failed: cudaError {rc}")
         return logits
 
     def make_plan(self, ids, cached, tables, lm_rows, slots=None):
@@ -904,6 +886,39 @@ class LlamaPrefill:
             p.dest_rows = ptr(6)
             p.runner_token_ids, p.runner_context_lens = runner.meta["token_ids"].data_ptr(), runner.context_lens.data_ptr()
         return p, logits, plan
+
+
+class LlamaPrefill(PromptPrefill):
+    """Prompt processing through `mrs_llama_prefill_step` (include/mrs_b200_model.h), the reference's prompt forward
+    (`models/llama.rs` Block::forward with seq_len > 1) over the packed rows of one or many sequences:
+    embedding -> per layer RMSNorm, wgmma dequant-GEMMs (grouped QKV, gate|up with the GLU epilogue), RoPE, var-len
+    causal prompt attention over the fresh q/k/v (the reference's flash-attn call, paged_attention.rs:1413-1475) and the
+    KV scatter into the paged HND cache, o_proj, add+RMSNorm, down, add+RMSNorm -> lm_head on each sequence's last row
+    (`extract_logits`) -> argmax.  A sequence with cached rows (prefix-cache hit, or a later chunk of a chunked prompt)
+    has its new K/V scattered first and attends over the cache (`prefill_attention_paged`).
+    `forward` is the one-sequence call; TTFT of BASELINE config 3 is its time on a 4096-token prompt.  `forward_batch`
+    runs up to 256 sequences in one step and can hand them to a decode runner's rows on the device."""
+    STEP = "mrs_llama_prefill_step"
+
+    def __init__(self, weights: "LlamaWeights", max_tokens=4096, runner: "LlamaRunner" = None, pdl=True):
+        """max_tokens: new rows per call (all sequences together); the scratch for them is allocated here.
+        runner: write prompts' K/V into this decode runner's paged cache (sequence 0's block table by default), so a
+        generation is prefill -> `runner.reset(T)` -> decode-graph replays, or `forward_batch(slots=...)` ->
+        decode-graph replays."""
+        from . import ops, paged_attn, quant  # noqa: F401  (fail early when the extension is missing)
+        if weights.tp_size != 1:
+            raise NotImplementedError("LlamaPrefill runs single-GPU")
+        self._init_caches(weights, max_tokens, runner)
+        cfg, dev, dt = self.cfg, self.dev, self.dt
+        T, H = self.max_tokens, cfg.hidden
+        nq, nkv = cfg.n_heads * cfg.head_dim, cfg.n_kv_heads * cfg.head_dim
+        a = lambda *s: torch.empty(*s, dtype=dt, device=dev)
+        self.buf = dict(x=a(T, H), x2=a(T, H), h=a(T, H), q=a(T, nq), k=a(T, nkv), v=a(T, nkv), attn_out=a(T, nq),
+                        act=a(T, cfg.inter), h_last=a(MAX_PREFILL_SEQS, H),
+                        gate_up=a(2, T, cfg.inter) if T > PREFILL_GROUPED_MAX_ROWS else None,
+                        argmax_scratch=torch.zeros(16 * MAX_PREFILL_SEQS + 16, dtype=torch.uint8, device=dev),
+                        q8_scratch=torch.empty(MMVQ_MAX_BATCH * (-(-H // 512) * 16) * 36, dtype=torch.uint8, device=dev))
+        self._layers, self.step_struct = _model_step(weights, self.k_cache, self.v_cache, pdl, cfg.n_heads, cfg.n_kv_heads)
 
 
 def check_drafts(drafts, batch, draft_len, vocab):
