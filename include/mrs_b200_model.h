@@ -272,6 +272,21 @@ int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream);
  * lm_rows != 1; paged outside 0..1, or paged 1 with the vLLM layout (the paged prompt kernel reads HND pages); an
  * activation dtype other than f16 / bf16; hidden % 8 != 0. */
 int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama_prefill *p, void *stream);
+/* Speculative decoding of a GPTQ / AWQ model: mrs_llama_verify_step's contract over the int4 layer stack.  s->batch = B
+ * sequences of q_len = k + 1 rows each (the anchor and k drafts); the metadata comes from mrs_decode_advance_multi.
+ * Every row buffer of `s` holds B*q_len rows: token_ids, positions, slot_mapping, x, x2, h, qkv, attn_out, o, gate_up,
+ * act, logits and out_token (which must not alias token_ids).  tmp_v / tmp_s hold [padded_tiles, q_len*n_heads(,
+ * head_dim)], attn_counters B*n_kv_heads*ceil(group*q_len/16) zeroed entries (left zero), argmax_scratch >= 16*B*q_len
+ * + 16 zeroed bytes.  Launches: the chain of mrs_gptq_decode_step over the B*q_len rows, with the same W4A16 GEMM
+ * flags (so plain and verify steps take one GEMM route), with mrs_paged_decode_fused_multi_strided reading q, k and v
+ * inside the q||k||v rows as the attention -> the dense lm_head on every row -> mrs_argmax into out_token ->
+ * mrs_spec_accept with `context_lens` (the lengths the advance read).  HND cache layout only: no multi-query kernel
+ * reads the vLLM layout.  Graph-capturable; skip_mask as for decode (bit 2 also takes mrs_spec_accept off the PDL
+ * chain).  cudaErrorInvalidValue, before any launch, for: B outside 1..256; q_len outside 2..8; cache_layout != 1; a
+ * head_dim other than 64 / 128; an activation dtype other than f16 / bf16; hidden % 8 != 0; a NULL s->layers;
+ * out_token == token_ids; a NULL context_lens, accepted or emitted. */
+int32_t mrs_gptq_verify_step(const mrs_gptq_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,
+                             int32_t *emitted, void *stream);
 /* The chain's links (not reference ABI): mrs_w4a16_gemm / mrs_dense_linear / add_rms_norm / fused_split_glu with a
  * `pdl` flag.  pdl bit 0 (value 1) makes the launch a link: it requires that the launch before it on `stream` is also a
  * link (or a plain kernel).  For mrs_w4a16_gemm_pdl and mrs_dense_linear_pdl, bit 1 (value 2) never splits K over a

@@ -125,6 +125,19 @@ int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_new, void *ke
                                float *tmp_s, int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
                                int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size, int32_t page_size,
                                float sm_scale, uint32_t dtype, int32_t pdl, int32_t q_len, void *stream);
+/* same with explicit row strides (elements) of q and of k_new / v_new, as mrs_paged_decode_fused_strided: a fused QKV
+ * GEMM writes [batch_size * q_len, (H + 2 KVH) D] and hands three pointers into it; o stays contiguous.  With the
+ * contiguous strides it is mrs_paged_decode_fused_multi. */
+int32_t mrs_paged_decode_fused_multi_strided(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
+                               const void *rope_cos, const void *rope_sin, const int32_t *positions,
+                               const int64_t *slot_mapping, const int32_t *kv_indptr, const int32_t *kv_indices,
+                               const int32_t *kv_last_page_len, const int32_t *request_indices,
+                               const int32_t *kv_tile_indices, const int32_t *o_indptr,
+                               const int32_t *kv_chunk_size_ptr, const uint8_t *block_valid_mask, void *o, void *tmp_v,
+                               float *tmp_s, int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
+                               int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size, int32_t page_size,
+                               float sm_scale, uint32_t dtype, int32_t pdl, int32_t q_len, int64_t q_stride_n,
+                               int64_t kv_new_stride, void *stream);
 /* ---- prompt attention over fresh q/k/v (SURVEY §8(f) rank 1; REF paged_attention.rs:1413-1475 ->
  * flash_attn_varlen): causal [+ sliding window / soft-cap], GQA, var-len batches via cu_seqlens
  * (device i32 [batch+1], or NULL for one sequence).  q [total,H,D], k/v [total,KVH,D], strides in

@@ -10,6 +10,8 @@
 //   add + RMSNorm -> gate||up GEMM -> SiLU*mul -> down GEMM -> add + RMSNorm (next layer's norm)
 // mrs_gptq_prefill_step runs the same chain over the packed prompt rows of up to 256 sequences, on whole-K GEMMs with
 // gate||up through the GLU epilogue, and the prompt attention of the Llama prompt step (prompt_step.cuh).
+// mrs_gptq_verify_step runs the decode chain over k + 1 rows per sequence (speculative decoding) with the multi-query
+// fused attention, then the greedy acceptance on the device.
 #include "common.cuh"
 #include "mrs_b200_model.h"
 #include "prompt_step.cuh"
@@ -79,14 +81,32 @@ extern "C" void mrs_add_rms_norm_pdl(const void *x, const void *residual, const 
 extern "C" void mrs_split_glu_pdl(const void *input, void *output, uint32_t rows, uint32_t split_size, int32_t activation,
                                   int32_t dtype, int32_t pdl, void *stream);
 
-extern "C" int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream) {
-  const int dt = s->act_dtype, B = s->batch, H = s->hidden;
+extern "C" int32_t mrs_paged_decode_fused_multi_strided(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
+                                                        const void *rope_cos, const void *rope_sin, const int32_t *positions,
+                                                        const int64_t *slot_mapping, const int32_t *kv_indptr,
+                                                        const int32_t *kv_indices, const int32_t *kv_last_page_len,
+                                                        const int32_t *request_indices, const int32_t *kv_tile_indices,
+                                                        const int32_t *o_indptr, const int32_t *kv_chunk_size_ptr,
+                                                        const uint8_t *block_valid_mask, void *o, void *tmp_v, float *tmp_s,
+                                                        int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
+                                                        int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
+                                                        int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
+                                                        int32_t q_len, int64_t q_stride_n, int64_t kv_new_stride,
+                                                        void *stream);
+extern "C" int32_t mrs_spec_accept(const int32_t *argmax, int32_t *token_ids, const int64_t *slot_mapping,
+                                   int32_t *context_lens, int32_t *accepted, int32_t *emitted, int32_t batch, int32_t q_len,
+                                   int32_t pdl, void *stream);
+
+// the decode layer chain + lm_head + argmax over s->batch sequences of q_len rows each (R = batch * q_len rows in every
+// row buffer): q_len == 1 is the decode step, q_len 2..8 a speculative verify step (HND layout only), whose attention is
+// the multi-query fused kernel reading q, k and v inside the q||k||v rows
+static int32_t gptq_forward(const mrs_gptq_step *s, int q_len, void *stream) {
+  const int dt = s->act_dtype, B = s->batch, R = B * q_len, H = s->hidden;
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim, nqkv = nq + 2 * nkv;
   cudaStream_t st = (cudaStream_t)stream;
-  if (B < 1 || B > 256 || (dt != MRS_F16 && dt != MRS_BF16) || H % 8) return (int32_t)cudaErrorInvalidValue;
   const bool f16 = dt == MRS_F16;
   auto rms = [&](const void *x, const void *w, void *dst) {
-    if (f16) mrs_rms_norm_f16(x, w, dst, B, H, s->rms_eps, (int64_t)stream); else mrs_rms_norm_bf16(x, w, dst, B, H, s->rms_eps, (int64_t)stream);
+    if (f16) mrs_rms_norm_f16(x, w, dst, R, H, s->rms_eps, (int64_t)stream); else mrs_rms_norm_bf16(x, w, dst, R, H, s->rms_eps, (int64_t)stream);
   };
   // Every launch of the layer loop is a link of ONE programmatic-dependent-launch chain (skip_mask bit 2 turns it
   // off): each kernel triggers its dependents when it starts and waits for the upstream grid before touching its
@@ -95,28 +115,38 @@ extern "C" int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream) {
   // so that layout keeps plain stream order.
   const int pdl = ((s->skip_mask & 4) || s->cache_layout != 1) ? 0 : 1;
   auto add_rms = [&](const void *x, const void *res, const void *w, void *res_dst, void *norm_dst) {
-    mrs_add_rms_norm_pdl(x, res, w, res_dst, norm_dst, B, H, s->rms_eps, dt, pdl, stream);
+    mrs_add_rms_norm_pdl(x, res, w, res_dst, norm_dst, R, H, s->rms_eps, dt, pdl, stream);
   };
+  // the same GEMM route for plain and verify steps: no whole-K bit, so both pick their K split by row count alone
   auto linear = [&](const mrs_w4_weight &w, const void *x, void *y) -> int {
-    return mrs_w4a16_gemm_pdl(x, w.tiles, w.scales, (const int32_t *)w.qzeros, y, B, w.k, w.n, s->group_size, dt, 0, pdl, stream);
+    return mrs_w4a16_gemm_pdl(x, w.tiles, w.scales, (const int32_t *)w.qzeros, y, R, w.k, w.n, s->group_size, dt, 0, pdl, stream);
   };
   const bool do_attn = !(s->skip_mask & 1), do_lin = !(s->skip_mask & 2);
+  void *tmp_v = s->padded_tiles > B ? s->tmp_v : nullptr;
+  float *tmp_s = s->padded_tiles > B ? s->tmp_s : nullptr;
+  const int rope_flags = (s->rope_neox ? 0 : 2) | pdl;
 
-  mrs::dense_embedding_kernel<<<B, 256, 0, st>>>((const uint4 *)s->tok_embd, H / 8, s->token_ids, (uint4 *)s->x);
+  mrs::dense_embedding_kernel<<<R, 256, 0, st>>>((const uint4 *)s->tok_embd, H / 8, s->token_ids, (uint4 *)s->x);
   void *x = s->x, *x2 = s->x2;   // residual stream ping-pong
   rms(x, s->layers[0].attn_norm, s->h);
   for (int l = 0; l < s->n_layers; l++) {
     const mrs_gptq_layer &L = s->layers[l];
     if (do_lin) MRS_TRY(linear(L.wqkv, s->h, s->qkv));
     void *q = s->qkv, *k = (char *)s->qkv + (size_t)nq * 2, *v = (char *)s->qkv + (size_t)(nq + nkv) * 2;
-    if (do_attn && s->cache_layout == 1) {
+    if (do_attn && q_len > 1) {
+      MRS_TRY(mrs_paged_decode_fused_multi_strided(q, k, v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
+                                                   s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
+                                                   s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
+                                                   s->block_valid_mask, s->attn_out, tmp_v, tmp_s, s->attn_counters, B,
+                                                   s->padded_tiles, s->n_heads, s->n_kv_heads, s->head_dim, s->block_size,
+                                                   s->sm_scale, (uint32_t)dt, rope_flags, q_len, nqkv, nqkv, stream));
+    } else if (do_attn && s->cache_layout == 1) {
       MRS_TRY(mrs_paged_decode_fused_strided(q, k, v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
                                              s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
                                              s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                                             s->block_valid_mask, s->attn_out, s->padded_tiles > B ? s->tmp_v : nullptr,
-                                             s->padded_tiles > B ? s->tmp_s : nullptr, s->attn_counters, B, s->padded_tiles,
-                                             s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
-                                             (s->rope_neox ? 0 : 2) | pdl, nqkv, nqkv, stream));
+                                             s->block_valid_mask, s->attn_out, tmp_v, tmp_s, s->attn_counters, B,
+                                             s->padded_tiles, s->n_heads, s->n_kv_heads, s->head_dim, s->block_size,
+                                             s->sm_scale, (uint32_t)dt, rope_flags, nqkv, nqkv, stream));
     } else if (do_attn) {
       // vLLM cache layout (REF MISTRALRS_FLASHINFER_DECODE=0): rotary -> reshape_and_cache -> paged_attention_v1
       rotary_embedding_positions(q, k, (void *)s->rope_cos, (void *)s->rope_sin, s->positions, s->rope_neox, s->head_dim, B,
@@ -138,14 +168,35 @@ extern "C" int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream) {
     if (do_lin) MRS_TRY(linear(L.wo, s->attn_out, s->o));
     add_rms(s->o, x, L.ffn_norm, x2, s->h);                                   // x2 = o + x ; h = norm(x2)
     if (do_lin) MRS_TRY(linear(L.w_gate_up, s->h, s->gate_up));
-    mrs_split_glu_pdl(s->gate_up, s->act, B, L.w_down.k, 0, dt, pdl, stream);
+    mrs_split_glu_pdl(s->gate_up, s->act, R, L.w_down.k, 0, dt, pdl, stream);
     if (do_lin) MRS_TRY(linear(L.w_down, s->act, s->o));
     const void *next_norm = (l + 1 < s->n_layers) ? s->layers[l + 1].attn_norm : s->final_norm;
     add_rms(s->o, x2, next_norm, x, s->h);                                     // x = down + x2 ; h = next norm(x)
   }
-  if (do_lin) MRS_TRY(mrs_dense_linear_pdl(s->h, s->lm_head, s->logits, B, H, s->vocab, dt, pdl, stream));
-  MRS_TRY(mrs_argmax(s->logits, B, s->vocab, dt, s->out_token, s->argmax_scratch, 0, stream));
+  if (do_lin) MRS_TRY(mrs_dense_linear_pdl(s->h, s->lm_head, s->logits, R, H, s->vocab, dt, pdl, stream));
+  MRS_TRY(mrs_argmax(s->logits, R, s->vocab, dt, s->out_token, s->argmax_scratch, 0, stream));
   return (int32_t)cudaGetLastError();
+}
+
+extern "C" int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream) {
+  const int dt = s->act_dtype, B = s->batch;
+  if (B < 1 || B > 256 || (dt != MRS_F16 && dt != MRS_BF16) || s->hidden % 8) return (int32_t)cudaErrorInvalidValue;
+  return gptq_forward(s, 1, stream);
+}
+
+// the verify step of speculative decoding (contract: include/mrs_b200_model.h): the decode chain over B * q_len rows,
+// then the greedy acceptance on the device, as mrs_llama_verify_step
+extern "C" int32_t mrs_gptq_verify_step(const mrs_gptq_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,
+                                        int32_t *emitted, void *stream) {
+  if (s == nullptr || s->batch < 1 || s->batch > 256 || q_len < 2 || q_len > 8 || s->cache_layout != 1 ||
+      (s->head_dim != 64 && s->head_dim != 128) || (s->act_dtype != MRS_F16 && s->act_dtype != MRS_BF16) ||
+      s->hidden % 8 != 0 || s->layers == nullptr || s->out_token == s->token_ids || context_lens == nullptr ||
+      accepted == nullptr || emitted == nullptr)
+    return (int32_t)cudaErrorInvalidValue;
+  MRS_TRY(gptq_forward(s, q_len, stream));
+  const int pdl = (s->skip_mask & 4) ? 0 : 1;
+  return mrs_spec_accept(s->out_token, s->token_ids, s->slot_mapping, context_lens, accepted, emitted, s->batch, q_len, pdl,
+                         stream);
 }
 
 // the prompt step over the packed rows of n sequences (contract: include/mrs_b200_model.h): the decode step's layer

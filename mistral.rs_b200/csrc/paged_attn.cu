@@ -966,6 +966,38 @@ extern "C" int32_t mrs_paged_decode_fused(void *q, void *k_new, void *v_new, voi
 // kv_len - q_len .. kv_len - 1, laid out [B * q_len, ...] in q / k_new / v_new / positions / slot_mapping / o;
 // partials tmp_v / tmp_s [padded_batch_size, q_len * num_qo_heads]; counters [B * KVH * ceil(group * q_len / 16)].
 // Head size 64 | 128, q_len 1..8, 16-bit dtypes.  A sequence needs kv_len >= q_len.
+// q rows are q_stride_n elements apart, k_new / v_new rows kv_new_stride (the [B * q_len, (H + 2 KVH) D] rows of a
+// fused QKV GEMM, as for mrs_paged_decode_fused_strided); o stays contiguous
+extern "C" int32_t mrs_paged_decode_fused_multi_strided(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
+                                                        const void *rope_cos, const void *rope_sin, const int32_t *positions,
+                                                        const int64_t *slot_mapping, const int32_t *kv_indptr,
+                                                        const int32_t *kv_indices, const int32_t *kv_last_page_len,
+                                                        const int32_t *request_indices, const int32_t *kv_tile_indices,
+                                                        const int32_t *o_indptr, const int32_t *kv_chunk_size_ptr,
+                                                        const uint8_t *block_valid_mask, void *o, void *tmp_v, float *tmp_s,
+                                                        int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
+                                                        int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
+                                                        int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
+                                                        int32_t q_len, int64_t q_stride_n, int64_t kv_new_stride,
+                                                        void *stream) {
+  if ((dtype != 0 && dtype != 1) || (head_size != 64 && head_size != 128) || q_len < 1 || q_len > 8 || num_kv_heads < 1 ||
+      num_qo_heads % num_kv_heads)
+    return (int32_t)cudaErrorInvalidValue;
+  PagedParams p = fused_decode_params(q, k_new, v_new, key_cache, value_cache, rope_cos, rope_sin, positions, slot_mapping,
+                                      kv_indptr, kv_indices, kv_last_page_len, request_indices, kv_tile_indices,
+                                      o_indptr, kv_chunk_size_ptr, block_valid_mask, o, tmp_v, tmp_s, counters,
+                                      batch_size, padded_batch_size, num_qo_heads, num_kv_heads, head_size,
+                                      page_size, sm_scale, pdl, q_stride_n, kv_new_stride);
+  p.q_len = q_len;
+  const int tiles = p.tmp_o != nullptr ? padded_batch_size : batch_size;
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e;
+  if (dtype == 0) e = head_size == 64 ? launch_decode_multi<__half, 64>(p, tiles, st) : launch_decode_multi<__half, 128>(p, tiles, st);
+  else e = head_size == 64 ? launch_decode_multi<__nv_bfloat16, 64>(p, tiles, st) : launch_decode_multi<__nv_bfloat16, 128>(p, tiles, st);
+  if (e != cudaSuccess) fprintf(stderr, "mrs_b200: mrs_paged_decode_fused_multi failed: %s\n", cudaGetErrorString(e));
+  return (int32_t)e;
+}
+
 extern "C" int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
                                                 const void *rope_cos, const void *rope_sin, const int32_t *positions,
                                                 const int64_t *slot_mapping, const int32_t *kv_indptr,
@@ -977,23 +1009,12 @@ extern "C" int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_ne
                                                 int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
                                                 int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
                                                 int32_t q_len, void *stream) {
-  if ((dtype != 0 && dtype != 1) || (head_size != 64 && head_size != 128) || q_len < 1 || q_len > 8 || num_kv_heads < 1 ||
-      num_qo_heads % num_kv_heads)
-    return (int32_t)cudaErrorInvalidValue;
-  PagedParams p = fused_decode_params(q, k_new, v_new, key_cache, value_cache, rope_cos, rope_sin, positions, slot_mapping,
-                                      kv_indptr, kv_indices, kv_last_page_len, request_indices, kv_tile_indices,
-                                      o_indptr, kv_chunk_size_ptr, block_valid_mask, o, tmp_v, tmp_s, counters,
-                                      batch_size, padded_batch_size, num_qo_heads, num_kv_heads, head_size,
-                                      page_size, sm_scale, pdl, (int64_t)num_qo_heads * head_size,
-                                      (int64_t)num_kv_heads * head_size);
-  p.q_len = q_len;
-  const int tiles = p.tmp_o != nullptr ? padded_batch_size : batch_size;
-  cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t e;
-  if (dtype == 0) e = head_size == 64 ? launch_decode_multi<__half, 64>(p, tiles, st) : launch_decode_multi<__half, 128>(p, tiles, st);
-  else e = head_size == 64 ? launch_decode_multi<__nv_bfloat16, 64>(p, tiles, st) : launch_decode_multi<__nv_bfloat16, 128>(p, tiles, st);
-  if (e != cudaSuccess) fprintf(stderr, "mrs_b200: mrs_paged_decode_fused_multi failed: %s\n", cudaGetErrorString(e));
-  return (int32_t)e;
+  return mrs_paged_decode_fused_multi_strided(q, k_new, v_new, key_cache, value_cache, rope_cos, rope_sin, positions,
+                                              slot_mapping, kv_indptr, kv_indices, kv_last_page_len, request_indices,
+                                              kv_tile_indices, o_indptr, kv_chunk_size_ptr, block_valid_mask, o, tmp_v, tmp_s,
+                                              counters, batch_size, padded_batch_size, num_qo_heads, num_kv_heads, head_size,
+                                              page_size, sm_scale, dtype, pdl, q_len, (int64_t)num_qo_heads * head_size,
+                                              (int64_t)num_kv_heads * head_size, stream);
 }
 
 // bit 0: keep HND decode attention on the SIMT kernel instead of the tensor-core one; bit 1: no cluster/DSMEM

@@ -17,7 +17,8 @@ import numpy as np
 import torch
 
 from . import lib
-from .model import MAX_PREFILL_SEQS, PagedDecodeRunner, PromptPrefill, _point, check_runner_args, rope_tables, runner_split_pages
+from .model import (MAX_PREFILL_SEQS, PagedDecodeRunner, PromptPrefill, SpecVerifier, _point, check_runner_args,
+                    rope_tables, runner_split_pages)
 
 
 @dataclass
@@ -236,3 +237,45 @@ class GptqPrefill(PromptPrefill):
             raise ValueError("GptqPrefill: cached rows need the HND cache layout (the paged prompt attention reads HND "
                              f"pages), the runner's is {self.layout!r}")
         return super().make_plan(ids, cached, tables, lm_rows, slots)
+
+
+def check_gptq_verifier_args(runner, draft_len):
+    """ValueError unless `runner` (a GptqRunner) can run verify steps of `draft_len` drafts (see GptqVerifier).  There is
+    no GEMV route in the GPTQ stack, so every batch 1..256 takes every draft_len 1..7."""
+    k = int(draft_len)
+    if not 1 <= k <= 7:
+        raise ValueError(f"draft_len must be 1..7, got {draft_len}")
+    if runner.layout != "hnd":
+        raise ValueError(f"verify steps need the HND cache layout (the multi-query attention reads HND pages), the "
+                         f"runner's is {runner.layout!r}")
+    if runner.cfg.head_dim not in (64, 128):
+        raise ValueError(f"verify attention supports head_dim 64 / 128, got {runner.cfg.head_dim}")
+    if runner.dt not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"verify steps run in f16 / bf16, got {runner.dt}")
+    if runner.max_ctx < k + 1:
+        raise ValueError(f"the runner's context ({runner.max_ctx}) is shorter than one verify step ({k + 1} rows)")
+    return k
+
+
+class GptqVerifier(SpecVerifier):
+    """Speculative decoding on a GptqRunner's sequences through `mrs_gptq_verify_step` (include/mrs_b200_model.h; see
+    SpecVerifier): the int4 layer stack over the B*q rows with the runner's GEMM route, the multi-query fused attention
+    reading q, k and v inside the q||k||v rows, the dense lm_head on every row, argmax and the acceptance.  Needs the
+    HND cache layout.  `speculative_generate` drives it as it drives a LlamaVerifier."""
+    STEP = "mrs_gptq_verify_step"
+
+    def __init__(self, runner: GptqRunner, draft_len: int):
+        k = check_gptq_verifier_args(runner, draft_len)
+        super().__init__(runner, k)
+        cfg, dev, dt, B, q = runner.cfg, runner.dev, runner.dt, self.B, self.q
+        R, D, KVH, NH, H, P = B * q, cfg.head_dim, cfg.n_kv_heads, cfg.n_heads, cfg.hidden, runner.padded_tiles
+        a = lambda *s: torch.zeros(*s, dtype=dt, device=dev)
+        z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=dev)
+        nsub = -(-(NH // KVH) * q // 16)
+        self.buf = dict(x=a(R, H), x2=a(R, H), h=a(R, H), qkv=a(R, (NH + 2 * KVH) * D), attn_out=a(R, NH * D),
+                        o=a(R, H), gate_up=a(R, 2 * cfg.inter), act=a(R, cfg.inter), logits=a(R, cfg.vocab),
+                        tmp_v=a(P, q * NH, D), tmp_s=z(P, q * NH, d=torch.float32), out_token=z(R),
+                        attn_counters=z(B * KVH * nsub), argmax_scratch=z(16 * R + 16, d=torch.uint8))
+        s = _Step.from_buffer_copy(runner.step_struct)   # weights, caches, shapes, tables, lengths: the runner's
+        _point(s, self.meta, self.buf)
+        self.step_struct = s

@@ -956,43 +956,31 @@ def check_verifier_args(runner, draft_len):
     return k
 
 
-class LlamaVerifier:
-    """Greedy speculative decoding on a LlamaRunner's sequences (REF mistralrs-core/src/speculative/): each verify step
+class SpecVerifier:
+    """Greedy speculative decoding on a decode runner's sequences (REF mistralrs-core/src/speculative/): each verify step
     feeds q = k + 1 rows per sequence — the anchor (the token the runner would process next) and k caller-proposed
-    drafts — through mrs_llama_verify_step in one pass over the weights, and accepts drafts on the device
-    (mrs_spec_accept).  Verify steps take the runner's linear route: the GEMV chain for 1..8 sequences (B * q <= 8),
-    the dequant-GEMM chain for 9..256 (B * q up to 2048 rows), so plain and verify steps share their numerics.
+    drafts — through the model's verify step in one pass over the weights, and accepts drafts on the device
+    (mrs_spec_accept).  This base holds what does not depend on the model: the B*q-row metadata over the runner's tables,
+    the accepted / emitted results and their pinned staging, the anchor hand-over, the advance, graph capture and
+    replay.  A subclass checks its arguments first, then calls this constructor, allocates its scratch (`buf`), points
+    its step struct (`step_struct`) and names its C entry (`STEP`), which forward() calls as
+    STEP(step, q, context_lens, accepted, emitted, stream).
 
     Shares the runner's weights, KV caches, block tables, context_lens and error_flag, so verify steps and plain
     `runner.step()` calls can be mixed; owns the B*q-row metadata and scratch.  The anchor moves explicitly:
     `sync_from_runner()` takes it from runner.meta["token_ids"], `sync_to_runner()` hands the next one back.  Rows a
     step rejected stay in the cache past the context and are overwritten later (never read)."""
+    STEP = None
 
-    def __init__(self, runner: LlamaRunner, draft_len: int):
-        k = check_verifier_args(runner, draft_len)
-        r, cfg, dev, dt = runner, runner.cfg, runner.dev, runner.dt
+    def __init__(self, runner, k):
+        """k: the checked draft length"""
         B, q = runner.B, k + 1
-        R = B * q
-        self.r, self.k, self.q, self.B, self.dev, self.vocab = runner, k, q, B, dev, cfg.vocab
-        z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=dev)
-        self.meta = r.decode_meta(q)
-        a = lambda *s: torch.zeros(*s, dtype=dt, device=dev)
-        H, D, n_heads, n_kv = cfg.hidden, cfg.head_dim, r.n_heads, r.n_kv
-        nsub = -(-(n_heads // n_kv) * q // 16)
-        self.buf = dict(x=a(R, H), x2=a(R, H), q=a(R, n_heads * D), k=a(R, n_kv * D), v=a(R, n_kv * D),
-                        attn_out=a(R, n_heads * D), act=a(R, cfg.inter), logits=a(R, cfg.vocab),
-                        tmp_v=a(r.padded_tiles, q * n_heads, D),
-                        tmp_s=torch.zeros(r.padded_tiles, q * n_heads, dtype=torch.float32, device=dev),
-                        out_token=z(R), attn_counters=z(B * n_kv * nsub),
-                        argmax_scratch=torch.zeros(16 * R + 16, dtype=torch.uint8, device=dev),
-                        h=a(R, H))                    # the GEMM route's normed activations (not the runner's [B, H])
-        self.results = z(B + R)                       # accepted [B] then emitted [B*q]: one D2H copy per step
-        self._results_h = torch.zeros(B + R, dtype=torch.int32).pin_memory()
+        self.r, self.k, self.q, self.B, self.dev, self.vocab = runner, k, q, B, runner.dev, runner.cfg.vocab
+        self.meta = runner.decode_meta(q)
+        self.results = torch.zeros(B + B * q, dtype=torch.int32, device=self.dev)   # accepted [B] then emitted [B*q]
+        self._results_h = torch.zeros(B + B * q, dtype=torch.int32).pin_memory()     # one D2H copy per step
         self._drafts_h = torch.zeros(B, k, dtype=torch.int32).pin_memory()
         self._h2d_done = torch.cuda.Event()
-        s = _Step.from_buffer_copy(runner.step_struct)   # weights, caches, shapes, pdl: the runner's
-        _point(s, self.meta, self.buf)
-        self.step_struct = s
         self.graph = None
 
     def sync_from_runner(self):
@@ -1013,17 +1001,22 @@ class LlamaVerifier:
         self.meta["token_ids"].view(self.B, self.q)[:, 1:].copy_(t, non_blocking=True)
         self._h2d_done.record()
 
+    def advance(self):
+        """enqueue the advance of every sequence by q rows (the metadata of the next verify step)"""
+        self.r._advance(self.meta, self.q)
+
     def forward(self):
+        """enqueue the verify step on the advanced metadata: the layer stack over the B*q rows, then the acceptance"""
         res = self.results
-        rc = lib().mrs_llama_verify_step(ctypes.byref(self.step_struct), ctypes.c_int(self.q),
-                                         ctypes.c_void_p(self.r.context_lens.data_ptr()), ctypes.c_void_p(res.data_ptr()),
-                                         ctypes.c_void_p(res.data_ptr() + 4 * self.B), self.r._stream())
+        rc = getattr(lib(), self.STEP)(ctypes.byref(self.step_struct), ctypes.c_int(self.q),
+                                       ctypes.c_void_p(self.r.context_lens.data_ptr()), ctypes.c_void_p(res.data_ptr()),
+                                       ctypes.c_void_p(res.data_ptr() + 4 * self.B), self.r._stream())
         if rc != 0:
-            raise RuntimeError(f"mrs_llama_verify_step failed: cudaError {rc}")
+            raise RuntimeError(f"{self.STEP} failed: cudaError {rc}")
 
     def step(self):
         """one verify step on the current anchors and drafts (eager): advance by q rows, verify, accept."""
-        self.r._advance(self.meta, self.q)
+        self.advance()
         self.forward()
 
     def capture(self):
@@ -1063,7 +1056,35 @@ class LlamaVerifier:
         return h[:self.B], [h[self.B + b * self.q:self.B + (b + 1) * self.q] for b in range(self.B)]
 
 
-def speculative_generate(verifier: LlamaVerifier, first_tokens, n_tokens, propose):
+class LlamaVerifier(SpecVerifier):
+    """Speculative decoding on a LlamaRunner's sequences through mrs_llama_verify_step (see SpecVerifier).  Verify
+    steps take the runner's linear route: the GEMV chain for 1..8 sequences (B * q <= 8), the dequant-GEMM chain for
+    9..256 (B * q up to 2048 rows), so plain and verify steps share their numerics."""
+    STEP = "mrs_llama_verify_step"
+
+    def __init__(self, runner: LlamaRunner, draft_len: int):
+        k = check_verifier_args(runner, draft_len)
+        super().__init__(runner, k)
+        r, cfg, dev, dt = runner, runner.cfg, runner.dev, runner.dt
+        B, q = self.B, self.q
+        R = B * q
+        z = lambda *s, d=torch.int32: torch.zeros(*s, dtype=d, device=dev)
+        a = lambda *s: torch.zeros(*s, dtype=dt, device=dev)
+        H, D, n_heads, n_kv = cfg.hidden, cfg.head_dim, r.n_heads, r.n_kv
+        nsub = -(-(n_heads // n_kv) * q // 16)
+        self.buf = dict(x=a(R, H), x2=a(R, H), q=a(R, n_heads * D), k=a(R, n_kv * D), v=a(R, n_kv * D),
+                        attn_out=a(R, n_heads * D), act=a(R, cfg.inter), logits=a(R, cfg.vocab),
+                        tmp_v=a(r.padded_tiles, q * n_heads, D),
+                        tmp_s=torch.zeros(r.padded_tiles, q * n_heads, dtype=torch.float32, device=dev),
+                        out_token=z(R), attn_counters=z(B * n_kv * nsub),
+                        argmax_scratch=torch.zeros(16 * R + 16, dtype=torch.uint8, device=dev),
+                        h=a(R, H))                    # the GEMM route's normed activations (not the runner's [B, H])
+        s = _Step.from_buffer_copy(runner.step_struct)   # weights, caches, shapes, pdl: the runner's
+        _point(s, self.meta, self.buf)
+        self.step_struct = s
+
+
+def speculative_generate(verifier: SpecVerifier, first_tokens, n_tokens, propose):
     """Greedy speculative generation: every sequence b starts from first_tokens[b] (processed at position
     runner.context_lens[b]) and runs until it has produced n_tokens tokens.  propose(history) -> k draft ids, where
     history is the sequence's tokens so far (first token included).  Per step: one pinned H2D copy of the drafts, one

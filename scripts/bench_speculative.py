@@ -79,10 +79,9 @@ def corruption_for(target, k):
     return (lo + hi) / 2
 
 
-def step_costs(runner, vers, linear, replays):
+def step_costs(runner, vers, linear, replays, ctx=PROMPT_LEN + GEN_LEN // 2):
     """step cost: plain decode and verify at q = k + 1 for every verifier, whole and split (`linear`: the name of the
-    linear-only split)"""
-    ctx = PROMPT_LEN + GEN_LEN // 2
+    linear-only split), every step at context `ctx`"""
     steps = {}
     for q in (1,) + tuple(k + 1 for k in vers):
         s = runner.step_struct if q == 1 else vers[q - 1].step_struct

@@ -1,7 +1,8 @@
-"""Print the kernel launches of the Llama decode, verify and prompt steps and of the GPTQ decode step, one line per kernel
-node of a captured CUDA graph, in dependency order: kernel name, grid, block, dynamic shared memory, cluster dimensions
-(when set) and whether the incoming edge is programmatic (a PDL link).  Two builds of libmrs_b200.so that print the same
-lines enqueue the same launches, so a refactor of host-side launch code can be checked against its parent:
+"""Print the kernel launches of the Llama decode, verify and prompt steps and of the GPTQ decode and verify steps, one
+line per kernel node of a captured CUDA graph, in dependency order: kernel name, grid, block, dynamic shared memory,
+cluster dimensions (when set) and whether the incoming edge is programmatic (a PDL link).  Two builds of libmrs_b200.so
+that print the same lines enqueue the same launches, so a refactor of host-side launch code can be checked against its
+parent:
 
     python scripts/launch_sequence.py > new.txt
     python scripts/launch_sequence.py --lib /path/to/parent/libmrs_b200.so > old.txt
@@ -167,6 +168,17 @@ def main():
             run.step()
             report(f"gptq decode {layout} B={B}", capture(run.step))
             del run
+    # ---- GPTQ verify steps (HND): advance_multi + W4A16 layer stack over B*q rows + lm_head + argmax + acceptance
+    for B, q in ((4, 4), (32, 8)):
+        run = G.GptqRunner(gw, batch=B, max_ctx=400)
+        run.set_tokens([(5 * b + 3) % 500 for b in range(B)])
+        run.step()
+        ver = G.GptqVerifier(run, draft_len=q - 1)
+        ver.sync_from_runner()
+        ver.set_drafts([[(b + i) % 500 for i in range(q - 1)] for b in range(B)])
+        ver.step()
+        report(f"gptq verify hnd B={B} q={q}", capture(ver.step))
+        del ver, run
     del gw
 
     # ---- verify steps: advance_multi + layer stack + lm_head + argmax + acceptance
