@@ -47,7 +47,8 @@ void mrs_set_pdl(int enabled);
 
 /* Tuning/diagnostic switches of the decode GEMV.  bit 3 (value 8): never use the long-K-segment
  * variant; bits 8.. : smallest stream (MiB of weights per launch) that takes it (default 128).
- * Both variants produce bit-identical results.  mrs_set_mmvq_ctas_per_sm: resident CTAs of one
+ * Both variants compute the same integer dots, but the long segments hand a block's chunks to other
+ * lanes, so an f32 output may differ in its last bit.  mrs_set_mmvq_ctas_per_sm: resident CTAs of one
  * launch per SM (1..3, default 2; 3 applies to batch 1). */
 void mrs_set_mmvq_flags(int flags);
 void mrs_set_mmvq_ctas_per_sm(int n);

@@ -224,8 +224,10 @@ __device__ __forceinline__ void lds_words_unaligned(const uint8_t *p, uint32_t (
 #pragma unroll
   for (int i = 0; i < N; i++) out[i] = __funnelshift_r(t[i], t[i + 1], sh);
 }
-__device__ __forceinline__ uint32_t lds_u16(const uint8_t *p) {  // 2-byte aligned
-  return *(const uint16_t *)p;
+// 16-bit read from shared memory: AL = 2-byte aligned, otherwise any byte alignment (a weight row at an odd address)
+template <bool AL> __device__ __forceinline__ uint32_t lds_u16(const uint8_t *p) {
+  if constexpr (AL) return *(const uint16_t *)p;
+  else return (uint32_t)p[0] | ((uint32_t)p[1] << 8);
 }
 
 __device__ __forceinline__ float half_bits_to_float(uint32_t h16) {

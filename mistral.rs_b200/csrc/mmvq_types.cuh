@@ -181,7 +181,7 @@ template <> struct QT<MRS_Q6_K> {
     const int8_t *sc = (const int8_t *)(blk + 192);
     const int is = 8 * n + 2 * (t >> 1) + (t & 1);
     w.sc_a = sc[is]; w.sc_b = sc[is + 4];
-    w.d = half_bits_to_float(lds_u16(blk + 208));
+    w.d = half_bits_to_float(lds_u16<AL>(blk + 208));
   }
   __device__ static __forceinline__ float dot(const W &w, const int *xq, const float *xa, int c) {
     const int sh = 2 * ((c & 3) >> 1);
@@ -277,7 +277,7 @@ template <> struct QT<MRS_Q3_K> {
       const int high = (s[8 + (is & 3)] >> (2 * (is >> 2))) & 3;
       w.sc[j] = (low | (high << 4)) - 32;
     }
-    w.d = half_bits_to_float(lds_u16(blk + 108));
+    w.d = half_bits_to_float(lds_u16<AL>(blk + 108));
   }
   __device__ static __forceinline__ float dot(const W &w, const int *xq, const float *xa, int c) {
     const int n = c >> 2;
@@ -313,7 +313,7 @@ template <> struct QT<MRS_Q8_0> {
   template <typename Y> __device__ static __forceinline__ void aux(const int *, int, Y y, float *a) { a[0] = y.d(0); }
   struct W { uint32_t q[8]; float d; };
   template <bool AL> __device__ static __forceinline__ void load(const uint8_t *blk, int, W &w) {
-    w.d = half_bits_to_float(lds_u16(blk));
+    w.d = half_bits_to_float(lds_u16<AL>(blk));
     lds_words_unaligned<8>(blk + 2, w.q);
   }
   __device__ static __forceinline__ float dot(const W &w, const int *xq, const float *xa, int) {
@@ -336,7 +336,7 @@ template <> struct QT<MRS_Q4_0> {
   template <typename Y> __device__ static __forceinline__ void aux(const int *, int, Y y, float *a) { a[0] = y.d(0); a[1] = y.s(0); }
   struct W { uint32_t q[4]; float d; };
   template <bool AL> __device__ static __forceinline__ void load(const uint8_t *blk, int, W &w) {
-    w.d = half_bits_to_float(lds_u16(blk));
+    w.d = half_bits_to_float(lds_u16<AL>(blk));
     lds_words_unaligned<4>(blk + 2, w.q);
   }
   __device__ static __forceinline__ float dot(const W &w, const int *xq, const float *xa, int) {
@@ -402,7 +402,7 @@ template <> struct QT<MRS_Q5_0> {
   template <typename Y> __device__ static __forceinline__ void aux(const int *, int, Y y, float *a) { a[0] = y.d(0); a[1] = y.s(0); }
   struct W { uint32_t q[4]; uint32_t qh; float d; };
   template <bool AL> __device__ static __forceinline__ void load(const uint8_t *blk, int, W &w) {
-    w.d = half_bits_to_float(lds_u16(blk));
+    w.d = half_bits_to_float(lds_u16<AL>(blk));
     uint32_t t[5];
     lds_words_unaligned<5>(blk + 2, t);
     w.qh = t[0];
