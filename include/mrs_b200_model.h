@@ -231,6 +231,14 @@ typedef struct {
   mrs_w4_weight wqkv, wo, w_gate_up, w_down;
   const void *attn_norm, *ffn_norm;
   void *k_cache, *v_cache;
+  /* act-order (GPTQ desc_act) row permutations of the linears, device int32 [K] each, NULL = natural order.  A linear
+   * repacked with `perm` (gptq_marlin_repack) holds checkpoint row perm[i] as its row i, so its input must arrive as
+   * x[:, perm].  perm_qkv: q, k and v share one (the norm in front of wqkv writes in that order: the first RMSNorm for
+   * layer 0, the previous layer's closing add + RMSNorm otherwise); perm_o: the attention output is gathered into
+   * attn_perm in that order before the o GEMM; perm_gate_up: gate and up share one (ffn_norm writes in that order).
+   * down_proj has no field: a loader permutes the N columns of gate and up by down's permutation instead, so the GLU
+   * output arrives in down's order.  The final norm is never permuted. */
+  const int32_t *perm_qkv, *perm_o, *perm_gate_up;
 } mrs_gptq_layer;
 typedef struct {
   int32_t hidden, n_layers, n_heads, n_kv_heads, head_dim, vocab, block_size, act_dtype, group_size;
@@ -245,8 +253,16 @@ typedef struct {
   int32_t *block_tables, *context_lens;    /* dense table + lengths (vLLM-layout attention) */
   void *x, *x2, *h, *qkv, *attn_out, *o, *gate_up, *act, *logits, *tmp_v; float *tmp_s;
   int32_t *out_token, *attn_counters; void *argmax_scratch;
+  void *attn_perm;                         /* [rows, n_heads*head_dim] act-order o_proj input, activation dtype; needed
+                                            * when any layer sets perm_o (NULL otherwise): rows = batch (decode step),
+                                            * batch*q_len (verify step), total_tokens (prompt step) */
 } mrs_gptq_step;
-/* skip_mask: bit0 skip rope/cache/attention, bit1 skip the linears (measurement only), bit2 plain stream order instead of
+/* Act-order layers (a perm_* field set) add launches to the chains below and change no other launch: the RMSNorm or
+ * add + RMSNorm in front of wqkv (w_gate_up) is mrs_rms_norm_perm_pdl / mrs_add_rms_norm_perm_pdl with perm_qkv
+ * (perm_gate_up), and mrs_gather_cols_pdl(attn_out -> attn_perm, perm_o) runs between the attention and the o GEMM as
+ * a link of the same chain.  Every step returns cudaErrorInvalidValue, before any launch, when a layer sets perm_o and
+ * attn_perm is NULL, or when a layer sets perm_qkv / perm_gate_up and hidden * 2 bytes exceed 48 KB.
+ * skip_mask: bit0 skip rope/cache/attention, bit1 skip the linears (measurement only), bit2 plain stream order instead of
  * the programmatic-dependent-launch chain (HND layout: every launch of the layer loop triggers its dependents at start
  * and waits for the upstream grid before touching its inputs/outputs, so each W4A16 GEMM streams weights while the
  * small kernel before it still runs). */
@@ -303,6 +319,20 @@ void mrs_add_rms_norm_pdl(const void *x, const void *residual, const void *weigh
                           int32_t nrows, int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream);
 void mrs_split_glu_pdl(const void *input, void *output, uint32_t rows, uint32_t split_size, int32_t activation,
                        int32_t dtype, int32_t pdl, void *stream);
+/* Norms in front of an act-order linear: the RMSNorm (mrs_rms_norm_f16 / _bf16) and the add + RMSNorm
+ * (mrs_add_rms_norm_pdl) with the normed output permuted, norm_dst[r, j] = norm[r, perm[j]] bit for bit, while
+ * residual_dst (the rounded sum x + residual) stays in natural order.  perm: device int32 [ncols], a permutation.  x may
+ * alias norm_dst (the row is staged in shared memory, so ncols * 2 bytes must not exceed 48 KB).  dtype f16 / bf16; pdl
+ * as above, 0 for the plain stream-ordered launch.  cudaErrorInvalidValue for a NULL perm (and, add form, a NULL
+ * residual or residual_dst), another dtype, or a row over 48 KB. */
+int32_t mrs_rms_norm_perm_pdl(const void *x, const void *weight, const int32_t *perm, void *norm_dst, int32_t nrows,
+                              int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream);
+int32_t mrs_add_rms_norm_perm_pdl(const void *x, const void *residual, const void *weight, const int32_t *perm,
+                                  void *residual_dst, void *norm_dst, int32_t nrows, int32_t ncols, float eps, int32_t dtype,
+                                  int32_t pdl, void *stream);
+/* Column gather of 16-bit rows: y[r, j] = x[r, perm[j]], x and y [rows, cols] contiguous and distinct; pdl as above. */
+int32_t mrs_gather_cols_pdl(const void *x, const int32_t *perm, void *y, int32_t rows, int32_t cols, int32_t pdl,
+                            void *stream);
 
 #ifdef __cplusplus
 }

@@ -149,6 +149,58 @@ static void launch_rms(const void *x, const void *res, const void *w, void *sum_
              (T *)sum_out, (T *)out, cols, eps, pdl);
 }
 
+// rms_norm_kernel with its normed output in the order of an act-order linear: out[j] = (the plain kernel's out)[perm[j]],
+// bit for bit (same block size, same per-thread sums, same rounding points); sum_out stays in natural order.  Thread j
+// reads element perm[j], which another thread loaded, so the row (the rounded sum when `res` is set) is staged in shared
+// memory: x may alias out (the prompt step normalises h in place), and nothing is re-read from global memory.
+template <typename T>
+__global__ void rms_norm_perm_kernel(const T *x, const T *res, const T *__restrict__ w, const int32_t *__restrict__ perm,
+                                     T *sum_out, T *out, int cols, float eps, int pdl) {
+  extern __shared__ __align__(16) unsigned char rms_row_smem[];
+  T *row = (T *)rms_row_smem;
+  __shared__ float red[32];
+  if (pdl) { pdl_launch_dependents(); pdl_wait(); }
+  const int64_t off = (int64_t)blockIdx.x * cols;
+  float ss = 0.f;
+  for (int c = threadIdx.x; c < cols; c += blockDim.x) {
+    T s;
+    if (res != nullptr) {
+      s = from_f<T>(to_f(x[off + c]) + to_f(res[off + c]));
+      sum_out[off + c] = s;
+    } else {
+      s = x[off + c];
+    }
+    row[c] = s;
+    const float v = to_f(s);
+    ss += v * v;
+  }
+  // block_sum's barriers also order every row[] store and every read of x before the first store to out
+  const float inv = rsqrtf(block_sum(ss, red) / (float)cols + eps);
+  for (int j = threadIdx.x; j < cols; j += blockDim.x) {
+    const int p = perm[j];
+    out[off + j] = from_f<T>(to_f(row[p]) * inv * to_f(w[p]));
+  }
+}
+
+template <typename T>
+static cudaError_t launch_rms_perm(const void *x, const void *res, const void *w, const int32_t *perm, void *sum_out, void *out,
+                                   int rows, int cols, float eps, cudaStream_t st, int pdl) {
+  if (rows <= 0 || cols <= 0) return cudaSuccess;
+  const size_t smem = (size_t)cols * sizeof(T);
+  if (perm == nullptr || smem > 48 * 1024) return cudaErrorInvalidValue;
+  const int block = cols < 1024 ? 128 : 512;     // as launch_rms: the same reduction, so the same inverse RMS
+  return launch_pdl(rms_norm_perm_kernel<T>, dim3(rows), dim3(block), smem, st, pdl, (const T *)x, (const T *)res,
+                    (const T *)w, perm, (T *)sum_out, (T *)out, cols, eps, pdl);
+}
+
+// y[r, j] = x[r, perm[j]] over 16-bit elements: the activations of an act-order linear whose input no norm produces
+__global__ void gather_cols_kernel(const uint16_t *__restrict__ x, const int32_t *__restrict__ perm, uint16_t *__restrict__ y,
+                                   int cols, int pdl) {
+  if (pdl) { pdl_launch_dependents(); pdl_wait(); }
+  const int64_t off = (int64_t)blockIdx.x * cols;
+  for (int j = threadIdx.x; j < cols; j += blockDim.x) y[off + j] = x[off + perm[j]];
+}
+
 // Per-head RMSNorm of a strided [B, H, S, D] view into a contiguous [B, H, S, D] tensor (QK-norm of
 // Qwen3 / Gemma-3 style models) — REF sort.cu:619-672 (one CTA per row there).  Here one warp per
 // row, eight rows per CTA: D is a head size (64..256), so a shuffle reduction is enough and a
@@ -247,6 +299,28 @@ extern "C" void mrs_add_rms_norm_pdl(const void *x, const void *residual, const 
                                      int32_t nrows, int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream) {
   if (dtype == MRS_F16) launch_rms<__half>(x, residual, weight, residual_dst, norm_dst, nrows, ncols, eps, (cudaStream_t)stream, pdl);
   else if (dtype == MRS_BF16) launch_rms<__nv_bfloat16>(x, residual, weight, residual_dst, norm_dst, nrows, ncols, eps, (cudaStream_t)stream, pdl);
+}
+// the norms in front of act-order linears (contract: include/mrs_b200_model.h); pdl 0 is the plain stream-ordered form
+extern "C" int32_t mrs_rms_norm_perm_pdl(const void *x, const void *weight, const int32_t *perm, void *norm_dst, int32_t nrows,
+                                         int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream) {
+  if (dtype == MRS_F16) return (int32_t)launch_rms_perm<__half>(x, nullptr, weight, perm, nullptr, norm_dst, nrows, ncols, eps, (cudaStream_t)stream, pdl);
+  if (dtype == MRS_BF16) return (int32_t)launch_rms_perm<__nv_bfloat16>(x, nullptr, weight, perm, nullptr, norm_dst, nrows, ncols, eps, (cudaStream_t)stream, pdl);
+  return (int32_t)cudaErrorInvalidValue;
+}
+extern "C" int32_t mrs_add_rms_norm_perm_pdl(const void *x, const void *residual, const void *weight, const int32_t *perm,
+                                             void *residual_dst, void *norm_dst, int32_t nrows, int32_t ncols, float eps,
+                                             int32_t dtype, int32_t pdl, void *stream) {
+  if (residual == nullptr || residual_dst == nullptr) return (int32_t)cudaErrorInvalidValue;
+  if (dtype == MRS_F16) return (int32_t)launch_rms_perm<__half>(x, residual, weight, perm, residual_dst, norm_dst, nrows, ncols, eps, (cudaStream_t)stream, pdl);
+  if (dtype == MRS_BF16) return (int32_t)launch_rms_perm<__nv_bfloat16>(x, residual, weight, perm, residual_dst, norm_dst, nrows, ncols, eps, (cudaStream_t)stream, pdl);
+  return (int32_t)cudaErrorInvalidValue;
+}
+extern "C" int32_t mrs_gather_cols_pdl(const void *x, const int32_t *perm, void *y, int32_t rows, int32_t cols, int32_t pdl,
+                                       void *stream) {
+  if (x == nullptr || perm == nullptr || y == nullptr || x == y || rows < 0 || cols < 0) return (int32_t)cudaErrorInvalidValue;
+  if (rows == 0 || cols == 0) return 0;
+  return (int32_t)launch_pdl(gather_cols_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, pdl, (const uint16_t *)x, perm,
+                             (uint16_t *)y, cols, pdl);
 }
 extern "C" void mrs_split_glu_pdl(const void *input, void *output, uint32_t rows, uint32_t split_size, int32_t activation,
                                   int32_t dtype, int32_t pdl, void *stream) {

@@ -8,6 +8,8 @@
 //   [RMSNorm] -> fused QKV GEMM -> RoPE + KV write + paged decode attention (one launch, HND; or the
 //   rotary -> reshape_and_cache -> paged_attention_v1 chain for the vLLM layout) -> o_proj GEMM ->
 //   add + RMSNorm -> gate||up GEMM -> SiLU*mul -> down GEMM -> add + RMSNorm (next layer's norm)
+// Act-order checkpoints (mrs_gptq_layer perm_* set): the norms in front of q||k||v and gate||up write their output in
+// the linear's row order, and a column gather of the attention output feeds o_proj; without them no launch changes.
 // mrs_gptq_prefill_step runs the same chain over the packed prompt rows of up to 256 sequences, on whole-K GEMMs with
 // gate||up through the GLU epilogue, and the prompt attention of the Llama prompt step (prompt_step.cuh).
 // mrs_gptq_verify_step runs the decode chain over k + 1 rows per sequence (speculative decoding) with the multi-query
@@ -80,6 +82,13 @@ extern "C" void mrs_add_rms_norm_pdl(const void *x, const void *residual, const 
                                      int32_t nrows, int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream);
 extern "C" void mrs_split_glu_pdl(const void *input, void *output, uint32_t rows, uint32_t split_size, int32_t activation,
                                   int32_t dtype, int32_t pdl, void *stream);
+extern "C" int32_t mrs_rms_norm_perm_pdl(const void *x, const void *weight, const int32_t *perm, void *norm_dst, int32_t nrows,
+                                         int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream);
+extern "C" int32_t mrs_add_rms_norm_perm_pdl(const void *x, const void *residual, const void *weight, const int32_t *perm,
+                                             void *residual_dst, void *norm_dst, int32_t nrows, int32_t ncols, float eps,
+                                             int32_t dtype, int32_t pdl, void *stream);
+extern "C" int32_t mrs_gather_cols_pdl(const void *x, const int32_t *perm, void *y, int32_t rows, int32_t cols, int32_t pdl,
+                                       void *stream);
 
 extern "C" int32_t mrs_paged_decode_fused_multi_strided(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
                                                         const void *rope_cos, const void *rope_sin, const int32_t *positions,
@@ -96,6 +105,19 @@ extern "C" int32_t mrs_paged_decode_fused_multi_strided(void *q, void *k_new, vo
 extern "C" int32_t mrs_spec_accept(const int32_t *argmax, int32_t *token_ids, const int64_t *slot_mapping,
                                    int32_t *context_lens, int32_t *accepted, int32_t *emitted, int32_t batch, int32_t q_len,
                                    int32_t pdl, void *stream);
+
+// act-order layers: every layer whose perm_o is set needs the attn_perm scratch, and a permuted norm stages a row of
+// `hidden` elements in shared memory
+static bool gptq_perms_ok(const mrs_gptq_step *s) {
+  if (s->layers == nullptr) return true;
+  bool any = false;
+  for (int l = 0; l < s->n_layers; l++) {
+    const mrs_gptq_layer &L = s->layers[l];
+    if (L.perm_o != nullptr && s->attn_perm == nullptr) return false;
+    any |= L.perm_qkv != nullptr || L.perm_gate_up != nullptr;
+  }
+  return !any || (size_t)s->hidden * 2 <= 48 * 1024;
+}
 
 // the decode layer chain + lm_head + argmax over s->batch sequences of q_len rows each (R = batch * q_len rows in every
 // row buffer): q_len == 1 is the decode step, q_len 2..8 a speculative verify step (HND layout only), whose attention is
@@ -114,8 +136,11 @@ static int32_t gptq_forward(const mrs_gptq_step *s, int q_len, void *stream) {
   // The HND attention launch is PDL-capable; the vLLM-layout chain (reference-ABI kernels, no PDL forms) is not,
   // so that layout keeps plain stream order.
   const int pdl = ((s->skip_mask & 4) || s->cache_layout != 1) ? 0 : 1;
-  auto add_rms = [&](const void *x, const void *res, const void *w, void *res_dst, void *norm_dst) {
+  // a norm whose consumer is an act-order linear writes its output in that linear's row order (perm != NULL)
+  auto add_rms = [&](const void *x, const void *res, const void *w, void *res_dst, void *norm_dst, const int32_t *perm) -> int {
+    if (perm != nullptr) return mrs_add_rms_norm_perm_pdl(x, res, w, perm, res_dst, norm_dst, R, H, s->rms_eps, dt, pdl, stream);
     mrs_add_rms_norm_pdl(x, res, w, res_dst, norm_dst, R, H, s->rms_eps, dt, pdl, stream);
+    return 0;
   };
   // the same GEMM route for plain and verify steps: no whole-K bit, so both pick their K split by row count alone
   auto linear = [&](const mrs_w4_weight &w, const void *x, void *y) -> int {
@@ -128,7 +153,10 @@ static int32_t gptq_forward(const mrs_gptq_step *s, int q_len, void *stream) {
 
   mrs::dense_embedding_kernel<<<R, 256, 0, st>>>((const uint4 *)s->tok_embd, H / 8, s->token_ids, (uint4 *)s->x);
   void *x = s->x, *x2 = s->x2;   // residual stream ping-pong
-  rms(x, s->layers[0].attn_norm, s->h);
+  if (s->layers[0].perm_qkv != nullptr)
+    MRS_TRY(mrs_rms_norm_perm_pdl(x, s->layers[0].attn_norm, s->layers[0].perm_qkv, s->h, R, H, s->rms_eps, dt, 0, stream));
+  else
+    rms(x, s->layers[0].attn_norm, s->h);
   for (int l = 0; l < s->n_layers; l++) {
     const mrs_gptq_layer &L = s->layers[l];
     if (do_lin) MRS_TRY(linear(L.wqkv, s->h, s->qkv));
@@ -165,13 +193,19 @@ static int32_t gptq_forward(const mrs_gptq_step *s, int q_len, void *stream) {
                                 s->max_blocks_per_seq * s->block_size, B, s->n_heads, s->head_dim, s->max_blocks_per_seq, nqkv,
                                 kv_block_stride, kv_head_stride, st, (uint32_t)dt, nullptr, nullptr, nullptr);
     }
-    if (do_lin) MRS_TRY(linear(L.wo, s->attn_out, s->o));
-    add_rms(s->o, x, L.ffn_norm, x2, s->h);                                   // x2 = o + x ; h = norm(x2)
+    const void *o_in = s->attn_out;
+    if (L.perm_o != nullptr) {                                                // o_proj's rows in act order
+      MRS_TRY(mrs_gather_cols_pdl(s->attn_out, L.perm_o, s->attn_perm, R, nq, pdl, stream));
+      o_in = s->attn_perm;
+    }
+    if (do_lin) MRS_TRY(linear(L.wo, o_in, s->o));
+    MRS_TRY(add_rms(s->o, x, L.ffn_norm, x2, s->h, L.perm_gate_up));          // x2 = o + x ; h = norm(x2)
     if (do_lin) MRS_TRY(linear(L.w_gate_up, s->h, s->gate_up));
     mrs_split_glu_pdl(s->gate_up, s->act, R, L.w_down.k, 0, dt, pdl, stream);
     if (do_lin) MRS_TRY(linear(L.w_down, s->act, s->o));
-    const void *next_norm = (l + 1 < s->n_layers) ? s->layers[l + 1].attn_norm : s->final_norm;
-    add_rms(s->o, x2, next_norm, x, s->h);                                     // x = down + x2 ; h = next norm(x)
+    const bool last = l + 1 == s->n_layers;
+    const void *next_norm = last ? s->final_norm : s->layers[l + 1].attn_norm;
+    MRS_TRY(add_rms(s->o, x2, next_norm, x, s->h, last ? nullptr : s->layers[l + 1].perm_qkv));   // x = down + x2 ; h = next norm(x)
   }
   if (do_lin) MRS_TRY(mrs_dense_linear_pdl(s->h, s->lm_head, s->logits, R, H, s->vocab, dt, pdl, stream));
   MRS_TRY(mrs_argmax(s->logits, R, s->vocab, dt, s->out_token, s->argmax_scratch, 0, stream));
@@ -180,7 +214,8 @@ static int32_t gptq_forward(const mrs_gptq_step *s, int q_len, void *stream) {
 
 extern "C" int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream) {
   const int dt = s->act_dtype, B = s->batch;
-  if (B < 1 || B > 256 || (dt != MRS_F16 && dt != MRS_BF16) || s->hidden % 8) return (int32_t)cudaErrorInvalidValue;
+  if (B < 1 || B > 256 || (dt != MRS_F16 && dt != MRS_BF16) || s->hidden % 8 || !gptq_perms_ok(s))
+    return (int32_t)cudaErrorInvalidValue;
   return gptq_forward(s, 1, stream);
 }
 
@@ -191,7 +226,7 @@ extern "C" int32_t mrs_gptq_verify_step(const mrs_gptq_step *s, int32_t q_len, i
   if (s == nullptr || s->batch < 1 || s->batch > 256 || q_len < 2 || q_len > 8 || s->cache_layout != 1 ||
       (s->head_dim != 64 && s->head_dim != 128) || (s->act_dtype != MRS_F16 && s->act_dtype != MRS_BF16) ||
       s->hidden % 8 != 0 || s->layers == nullptr || s->out_token == s->token_ids || context_lens == nullptr ||
-      accepted == nullptr || emitted == nullptr)
+      accepted == nullptr || emitted == nullptr || !gptq_perms_ok(s))
     return (int32_t)cudaErrorInvalidValue;
   MRS_TRY(gptq_forward(s, q_len, stream));
   const int pdl = (s->skip_mask & 4) ? 0 : 1;
@@ -222,6 +257,7 @@ extern "C" int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama
   if (p->lm_rows == 2 && p->logits == nullptr) return (int32_t)cudaErrorInvalidValue;
   if (p->dest_rows != nullptr && (p->runner_token_ids == nullptr || p->runner_context_lens == nullptr))
     return (int32_t)cudaErrorInvalidValue;
+  if (!gptq_perms_ok(s)) return (int32_t)cudaErrorInvalidValue;
 
   const int nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim, nqkv = nq + 2 * nkv;
   // the attention launches are plain kernels, which a PDL link may follow: the GEMMs and norms are links in both layouts
@@ -231,14 +267,19 @@ extern "C" int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama
     return mrs_w4a16_gemm_pdl(x, w.tiles, w.scales, (const int32_t *)w.qzeros, y, T, w.k, w.n, s->group_size, dt, 0,
                               pdl | 2 | flags, stream);
   };
-  auto add_rms = [&](const void *res, const void *w, void *res_dst) {   // res_dst = h + res ; h = norm(res_dst)
+  // res_dst = h + res ; h = norm(res_dst), in the row order of the act-order linear after it when perm != NULL
+  auto add_rms = [&](const void *res, const void *w, void *res_dst, const int32_t *perm) -> int32_t {
+    if (perm != nullptr) return mrs_add_rms_norm_perm_pdl(p->h, res, w, perm, res_dst, p->h, T, H, s->rms_eps, dt, pdl, stream);
     mrs_add_rms_norm_pdl(p->h, res, w, res_dst, p->h, T, H, s->rms_eps, dt, pdl, stream);
+    return 0;
   };
   const PromptAttnModel am{s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->rope_neox, dt, s->sm_scale, s->rope_cos,
                            s->rope_sin};
 
   mrs::dense_embedding_kernel<<<T, 256, 0, (cudaStream_t)stream>>>((const uint4 *)s->tok_embd, H / 8, p->token_ids, (uint4 *)p->x);
-  if (dt == MRS_F16) mrs_rms_norm_f16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
+  if (s->layers[0].perm_qkv != nullptr)
+    MRS_TRY(mrs_rms_norm_perm_pdl(p->x, s->layers[0].attn_norm, s->layers[0].perm_qkv, p->h, T, H, s->rms_eps, dt, 0, stream));
+  else if (dt == MRS_F16) mrs_rms_norm_f16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
   else mrs_rms_norm_bf16(p->x, s->layers[0].attn_norm, p->h, T, H, s->rms_eps, (int64_t)stream);
   for (int l = 0; l < s->n_layers; l++) {
     const mrs_gptq_layer &L = s->layers[l];
@@ -246,11 +287,18 @@ extern "C" int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama
     void *q = p->q, *k = (char *)p->q + (size_t)nq * 2, *v = (char *)p->q + (size_t)(nq + nkv) * 2;
     MRS_TRY(prompt_attention(p, am, q, k, v, nqkv, nqkv, L.k_cache, L.v_cache, vllm_cache, stream));
     // the o and down GEMMs write into h, which the add + RMSNorm after them reads as its input and overwrites
-    MRS_TRY(linear(L.wo, p->attn_out, p->h, 0));
-    add_rms(p->x, L.ffn_norm, p->x2);                                        // x2 = o + x ; h = norm(x2)
+    const void *o_in = p->attn_out;
+    if (L.perm_o != nullptr) {                                                // o_proj's rows in act order: [T, nq] scratch
+      MRS_TRY(mrs_gather_cols_pdl(p->attn_out, L.perm_o, s->attn_perm, T, nq, pdl, stream));
+      o_in = s->attn_perm;
+    }
+    MRS_TRY(linear(L.wo, o_in, p->h, 0));
+    MRS_TRY(add_rms(p->x, L.ffn_norm, p->x2, L.perm_gate_up));               // x2 = o + x ; h = norm(x2)
     MRS_TRY(linear(L.w_gate_up, p->h, p->act, 4));                           // act = silu(gate) * up
     MRS_TRY(linear(L.w_down, p->act, p->h, 0));
-    add_rms(p->x2, l + 1 < s->n_layers ? s->layers[l + 1].attn_norm : s->final_norm, p->x);   // x = down + x2 ; h = next norm(x)
+    const bool last = l + 1 == s->n_layers;
+    MRS_TRY(add_rms(p->x2, last ? s->final_norm : s->layers[l + 1].attn_norm, p->x,
+                    last ? nullptr : s->layers[l + 1].perm_qkv));            // x = down + x2 ; h = next norm(x)
   }
   if (p->lm_rows == 2) {
     MRS_TRY(mrs_dense_linear_pdl(p->h, s->lm_head, p->logits, T, H, s->vocab, dt, pdl | 2, stream));
