@@ -265,7 +265,11 @@ typedef struct {
  * skip_mask: bit0 skip rope/cache/attention, bit1 skip the linears (measurement only), bit2 plain stream order instead of
  * the programmatic-dependent-launch chain (HND layout: every launch of the layer loop triggers its dependents at start
  * and waits for the upstream grid before touching its inputs/outputs, so each W4A16 GEMM streams weights while the
- * small kernel before it still runs). */
+ * small kernel before it still runs).
+ * mrs_gptq_decode_step: the chain above over s->batch rows, the dense lm_head and mrs_argmax into out_token.
+ * cudaErrorInvalidValue, before any launch, for: a NULL s; batch outside 1..256; an activation dtype other than
+ * f16 / bf16; hidden % 8 != 0; a NULL s->layers or n_layers < 1; cache_layout outside 0..1; the act-order faults above.
+ * The verify step below rejects all of these too, and so does the prompt step, with the plan's n in place of batch. */
 int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream);
 /* Batched prompt prefill of a GPTQ / AWQ model: mrs_llama_prefill_step's contract over the int4 layer stack.  `s` gives
  * weights, norms, per-layer caches (in s->cache_layout), dims, activation dtype, group size, RoPE tables and rope_neox;
@@ -286,7 +290,7 @@ int32_t mrs_gptq_decode_step(const mrs_gptq_step *s, void *stream);
  * last_rows, h_last, logits, out_token and argmax_scratch when lm_rows == 1; logits when lm_rows == 2;
  * runner_token_ids and runner_context_lens when dest_rows is set); lm_rows outside 0..2; dest_rows set while
  * lm_rows != 1; paged outside 0..1, or paged 1 with the vLLM layout (the paged prompt kernel reads HND pages); an
- * activation dtype other than f16 / bf16; hidden % 8 != 0. */
+ * activation dtype other than f16 / bf16; hidden % 8 != 0; n_layers < 1; cache_layout outside 0..1. */
 int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama_prefill *p, void *stream);
 /* Speculative decoding of a GPTQ / AWQ model: mrs_llama_verify_step's contract over the int4 layer stack.  s->batch = B
  * sequences of q_len = k + 1 rows each (the anchor and k drafts); the metadata comes from mrs_decode_advance_multi.
@@ -299,8 +303,8 @@ int32_t mrs_gptq_prefill_step(const mrs_gptq_step *s, const mrs_llama_prefill *p
  * mrs_spec_accept with `context_lens` (the lengths the advance read).  HND cache layout only: no multi-query kernel
  * reads the vLLM layout.  Graph-capturable; skip_mask as for decode (bit 2 also takes mrs_spec_accept off the PDL
  * chain).  cudaErrorInvalidValue, before any launch, for: B outside 1..256; q_len outside 2..8; cache_layout != 1; a
- * head_dim other than 64 / 128; an activation dtype other than f16 / bf16; hidden % 8 != 0; a NULL s->layers;
- * out_token == token_ids; a NULL context_lens, accepted or emitted. */
+ * head_dim other than 64 / 128; an activation dtype other than f16 / bf16; hidden % 8 != 0; a NULL s->layers or
+ * n_layers < 1; out_token == token_ids; a NULL context_lens, accepted or emitted. */
 int32_t mrs_gptq_verify_step(const mrs_gptq_step *s, int32_t q_len, int32_t *context_lens, int32_t *accepted,
                              int32_t *emitted, void *stream);
 /* The chain's links (not reference ABI): mrs_w4a16_gemm / mrs_dense_linear / add_rms_norm / fused_split_glu with a

@@ -9,98 +9,9 @@
 #include "common.cuh"
 #include "dequant.cuh"
 #include "mrs_b200_model.h"
-#include "prompt_step.cuh"
-
-
-extern "C" int mrs_mmvq_fused(int ggml_type, int mode, int dt, const void *w0, const void *w1, const void *w2,
-                              const void *x, const void *norm_w, float eps, const void *residual, void *dst0,
-                              void *dst1, void *dst2, int K, int n0, int n1, int n2, int b_size, int activation,
-                              int pdl, void *stream);
-extern "C" int mrs_mmvq_fused_qkv_mixed(int type_qk, int type_v, int dt, const void *wq, const void *wk, const void *wv,
-                                        const void *x, const void *norm_w, float eps, void *q, void *k, void *v,
-                                        int K, int nq, int nk, int nv, int b_size, int pdl, void *stream);
-extern "C" int32_t mrs_mmq_gguf(int32_t ggml_type, const void *w, const void *x, void *y, int32_t M, int32_t N, int32_t K,
-                                int32_t dtype, void *stream);
-extern "C" int32_t mrs_mmq_gguf_grouped(int32_t ggml_type, int32_t n_mats, const void **w, const int32_t *rows,
-                                        void **y, const void *x, int32_t M, int32_t K, int32_t dtype, int32_t glu,
-                                        int32_t pdl, void *stream);
-extern "C" void mrs_rms_norm_f16(const void *x, const void *weight, void *dst, const int nrows, const int ncols, const float eps, int64_t stream);
-extern "C" void mrs_rms_norm_bf16(const void *x, const void *weight, void *dst, const int nrows, const int ncols, const float eps, int64_t stream);
-extern "C" void mrs_add_rms_norm_pdl(const void *x, const void *residual, const void *weight, void *residual_dst, void *norm_dst,
-                                     int32_t nrows, int32_t ncols, float eps, int32_t dtype, int32_t pdl, void *stream);
-extern "C" void rotary_embedding_positions(void *query, void *key, void *cos_cache, void *sin_cache, void *positions,
-                                           int32_t is_neox, int32_t head_size, int64_t num_tokens, int32_t rot_dim,
-                                           int32_t seq_len, int32_t num_heads, int32_t num_kv_heads,
-                                           int64_t query_stride, int64_t key_stride, uint32_t dtype, int64_t stream);
-extern "C" void reshape_and_cache_flashinfer(void *key, void *value, void *key_cache, void *value_cache,
-                                             int64_t *slot_mapping, int32_t num_tokens, int32_t num_heads,
-                                             int32_t head_size, int32_t block_size, int32_t key_stride,
-                                             int32_t value_stride, float k_scale, float v_scale, uint32_t dtype,
-                                             uint32_t cache_dtype, cudaStream_t stream);
-extern "C" void reshape_and_cache(void *key, void *value, void *key_cache, void *value_cache, int64_t *slot_mapping,
-                                  int32_t num_tokens, int32_t num_heads, int32_t head_size, int32_t block_size, int32_t x,
-                                  int32_t key_stride, int32_t value_stride, cudaStream_t stream, uint32_t dtype,
-                                  uint32_t cache_dtype, float *k_scale, float *v_scale);
-extern "C" int32_t mrs_paged_decode_fused(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
-                                          const void *rope_cos, const void *rope_sin, const int32_t *positions,
-                                          const int64_t *slot_mapping, const int32_t *kv_indptr,
-                                          const int32_t *kv_indices, const int32_t *kv_last_page_len,
-                                          const int32_t *request_indices, const int32_t *kv_tile_indices,
-                                          const int32_t *o_indptr, const int32_t *kv_chunk_size_ptr,
-                                          const uint8_t *block_valid_mask, void *o, void *tmp_v, float *tmp_s,
-                                          int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
-                                          int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
-                                          int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
-                                          void *stream);
-extern "C" int32_t mrs_paged_decode_fused_multi(void *q, void *k_new, void *v_new, void *key_cache, void *value_cache,
-                                                const void *rope_cos, const void *rope_sin, const int32_t *positions,
-                                                const int64_t *slot_mapping, const int32_t *kv_indptr,
-                                                const int32_t *kv_indices, const int32_t *kv_last_page_len,
-                                                const int32_t *request_indices, const int32_t *kv_tile_indices,
-                                                const int32_t *o_indptr, const int32_t *kv_chunk_size_ptr,
-                                                const uint8_t *block_valid_mask, void *o, void *tmp_v, float *tmp_s,
-                                                int32_t *counters, int32_t batch_size, int32_t padded_batch_size,
-                                                int32_t num_qo_heads, int32_t num_kv_heads, int32_t head_size,
-                                                int32_t page_size, float sm_scale, uint32_t dtype, int32_t pdl,
-                                                int32_t q_len, void *stream);
-extern "C" int32_t flashinfer_decode(void *q, void *key_cache, void *value_cache, const int32_t *kv_indptr,
-                                     const int32_t *kv_indices, const int32_t *kv_last_page_len,
-                                     const int32_t *request_indices, const int32_t *kv_tile_indices,
-                                     const int32_t *o_indptr, const int32_t *kv_chunk_size_ptr,
-                                     const bool *block_valid_mask, void *o, void *tmp_v, void *tmp_s,
-                                     int32_t batch_size, int32_t padded_batch_size, int32_t num_qo_heads,
-                                     int32_t num_kv_heads, int32_t head_size, int32_t page_size, int32_t q_stride_n,
-                                     int32_t q_stride_h, float sm_scale, int32_t window_left, float logits_soft_cap,
-                                     float k_scale, float v_scale, uint32_t dtype, uint32_t cache_dtype,
-                                     cudaStream_t stream);
-
-extern "C" int32_t mrs_prefill_attention(const void *q, const void *k, const void *v, void *out, const int32_t *cu_seqlens,
-                                         int32_t batch, int32_t total_tokens, int32_t max_seqlen, int32_t num_heads,
-                                         int32_t num_kv_heads, int32_t head_dim, int64_t q_stride, int64_t kv_stride,
-                                         int64_t o_stride, float softmax_scale, int32_t causal, int32_t window_left,
-                                         float softcap, uint32_t dtype, void *stream);
-extern "C" int32_t mrs_prefill_attention_paged(const void *q, const void *key_cache, const void *value_cache, void *out,
-                                               const int32_t *block_table, int32_t block_table_stride,
-                                               const int32_t *cu_seqlens_q, const int32_t *cu_seqlens_k, int32_t batch,
-                                               int32_t total_q, int32_t max_seqlen_q, int32_t max_seqlen_k, int32_t num_blocks,
-                                               int32_t num_heads, int32_t num_kv_heads, int32_t head_dim, int32_t page_size,
-                                               int64_t q_stride, int64_t o_stride, float softmax_scale, int32_t causal,
-                                               int32_t window_left, float softcap, uint32_t dtype, void *stream);
-extern "C" void fused_glu_f16(const void *a, const void *b, void *output, uint32_t rows, uint32_t cols, uint32_t a_row_stride,
-                              uint32_t b_row_stride, int activation, cudaStream_t stream);
-extern "C" void fused_glu_bf16(const void *a, const void *b, void *output, uint32_t rows, uint32_t cols, uint32_t a_row_stride,
-                               uint32_t b_row_stride, int activation, cudaStream_t stream);
-// the reference-shaped MMVQ launchers (mmvq.cu) the n <= 8 prompt lm_head issues, as `quant.plain` / fast_mmvq plain
-extern "C" void launch_mmvq_gguf_quantize_q8_1_bf16(const void *x, void *vy, int kx, int kx_padded, int num_rows, void *stream);
-extern "C" void launch_mmvq_gguf_quantize_q8_1_f16(const void *x, void *vy, int kx, int kx_padded, int num_rows, void *stream);
-#define MRS_PLAIN_DECL(tag)                                                                                             \
-  extern "C" void launch_mmvq_gguf_##tag##_bf16_plain(const void *vx, const void *vy, void *dst, int ncols_x, int nrows_x, \
-                                                      int stride_col_y, int stride_col_dst, int b_size, void *stream);    \
-  extern "C" void launch_mmvq_gguf_##tag##_f16_plain(const void *vx, const void *vy, void *dst, int ncols_x, int nrows_x,  \
-                                                     int stride_col_y, int stride_col_dst, int b_size, void *stream);
-MRS_PLAIN_DECL(q4_0) MRS_PLAIN_DECL(q4_1) MRS_PLAIN_DECL(q5_0) MRS_PLAIN_DECL(q5_1) MRS_PLAIN_DECL(q8_0)
-MRS_PLAIN_DECL(q2_k) MRS_PLAIN_DECL(q3_k) MRS_PLAIN_DECL(q4_k) MRS_PLAIN_DECL(q5_k) MRS_PLAIN_DECL(q6_k)
-#undef MRS_PLAIN_DECL
+#include "mrs_b200_ops.h"
+#include "mrs_b200_quant.h"
+#include "step_common.cuh"
 
 namespace mrs {
 
@@ -388,7 +299,25 @@ __global__ void prefill_commit_kernel(const int32_t *__restrict__ out_token, con
   context_lens[r] = cu_k[i + 1] - cu_k[i];
 }
 
-// ---- the prompt-step parts shared with the GPTQ prompt step (prompt_step.cuh)
+// ---- the prompt-step parts shared with the GPTQ prompt step (step_common.cuh)
+bool prompt_plan_ok(const mrs_llama_prefill *p, int act_dtype, int hidden) {
+  const int n = p->n_seqs;
+  if (n < 1 || n > 256 || p->total_tokens < n || (act_dtype != MRS_F16 && act_dtype != MRS_BF16) || p->lm_rows < 0 ||
+      p->lm_rows > 2 || (p->paged != 0 && p->paged != 1) || (p->dest_rows != nullptr && p->lm_rows != 1) ||
+      p->max_q_len < 1 || p->max_kv_len < p->max_q_len || hidden % 8 != 0)
+    return false;
+  if (p->token_ids == nullptr || p->positions == nullptr || p->slot_mapping == nullptr || p->cu_seqlens_q == nullptr ||
+      p->cu_seqlens_k == nullptr || p->x == nullptr || p->x2 == nullptr || p->h == nullptr || p->q == nullptr ||
+      p->attn_out == nullptr || p->act == nullptr)
+    return false;
+  if (p->paged && (p->block_tables == nullptr || p->block_table_stride < 1 || p->num_blocks < 1)) return false;
+  if (p->lm_rows == 1 && (p->last_rows == nullptr || p->h_last == nullptr || p->logits == nullptr || p->out_token == nullptr ||
+                          p->argmax_scratch == nullptr))
+    return false;
+  if (p->lm_rows == 2 && p->logits == nullptr) return false;
+  return p->dest_rows == nullptr || (p->runner_token_ids != nullptr && p->runner_context_lens != nullptr);
+}
+
 int32_t prompt_attention(const mrs_llama_prefill *p, const PromptAttnModel &m, void *q, void *k, void *v, int64_t q_stride,
                          int64_t kv_stride, void *k_cache, void *v_cache, bool vllm_cache, void *stream) {
   const int n = p->n_seqs, T = p->total_tokens, dt = m.act_dtype, nq = m.n_heads * m.head_dim;
@@ -530,26 +459,14 @@ static int32_t check_model(const mrs_llama_step *s) {
   return 0;
 }
 
-// the decode attention of layer L over s->batch sequences of q_len rows each: mrs_paged_decode_fused_multi for a verify
-// step (q_len > 1), else mrs_paged_decode_fused, or with fused_attention == 0 the RoPE -> KV scatter -> paged decode chain
+// the decode attention of layer L over s->batch sequences of q_len rows each: the fused kernel (multi-query for a verify
+// step, q_len > 1), or with fused_attention == 0 the RoPE -> KV scatter -> paged decode chain
 static int32_t decode_attention(const mrs_llama_step *s, const mrs_llama_layer &L, int q_len, void *stream) {
   const int B = s->batch, dt = s->act_dtype, nq = s->n_heads * s->head_dim, nkv = s->n_kv_heads * s->head_dim;
-  const int flags = s->pdl | (s->rope_neox ? 0 : 2);
+  if (q_len > 1 || s->fused_attention)
+    return fused_decode_attention(s, L.k_cache, L.v_cache, s->q, s->k, s->v, nq, nkv, q_len, s->pdl, stream);
   void *tmp_v = s->padded_tiles > B ? s->tmp_v : nullptr;
   float *tmp_s = s->padded_tiles > B ? s->tmp_s : nullptr;
-  if (q_len > 1)
-    return mrs_paged_decode_fused_multi(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
-                                        s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len,
-                                        s->request_indices, s->kv_tile_indices, s->o_indptr, s->kv_chunk_size,
-                                        s->block_valid_mask, s->attn_out, tmp_v, tmp_s, s->attn_counters, B, s->padded_tiles,
-                                        s->n_heads, s->n_kv_heads, s->head_dim, s->block_size, s->sm_scale, (uint32_t)dt,
-                                        flags, q_len, stream);
-  if (s->fused_attention)
-    return mrs_paged_decode_fused(s->q, s->k, s->v, L.k_cache, L.v_cache, s->rope_cos, s->rope_sin, s->positions,
-                                  s->slot_mapping, s->kv_indptr, s->kv_indices, s->kv_last_page_len, s->request_indices,
-                                  s->kv_tile_indices, s->o_indptr, s->kv_chunk_size, s->block_valid_mask, s->attn_out, tmp_v,
-                                  tmp_s, s->attn_counters, B, s->padded_tiles, s->n_heads, s->n_kv_heads, s->head_dim,
-                                  s->block_size, s->sm_scale, (uint32_t)dt, flags, stream);
   rotary_embedding_positions(s->q, s->k, (void *)s->rope_cos, (void *)s->rope_sin, s->positions, s->rope_neox, s->head_dim,
                              B, s->head_dim / 2, 0, s->n_heads, s->n_kv_heads, nq, nkv, (uint32_t)dt, (int64_t)stream);
   reshape_and_cache_flashinfer(s->k, s->v, L.k_cache, L.v_cache, s->slot_mapping, B, s->n_kv_heads, s->head_dim,
@@ -772,23 +689,10 @@ extern "C" int32_t mrs_llama_verify_step(const mrs_llama_step *s, int32_t q_len,
 // the prompt step over the packed rows of n sequences (contract: include/mrs_b200_model.h): the GEMM layer chain over T
 // rows with whole K, with the var-len prompt attention instead of the decode attention
 extern "C" int32_t mrs_llama_prefill_step(const mrs_llama_step *s, const mrs_llama_prefill *p, void *stream) {
-  if (s == nullptr || p == nullptr) return (int32_t)cudaErrorInvalidValue;
+  if (s == nullptr || p == nullptr || !prompt_plan_ok(p, s->act_dtype, s->hidden)) return (int32_t)cudaErrorInvalidValue;
   const int n = p->n_seqs, T = p->total_tokens, dt = s->act_dtype, H = s->hidden, pdl = s->pdl;
-  if (n < 1 || n > 256 || T < n || (dt != MRS_F16 && dt != MRS_BF16) || s->tp != nullptr || s->all_reduce != nullptr ||
-      p->lm_rows < 0 || p->lm_rows > 2 || (p->paged != 0 && p->paged != 1) || (p->dest_rows != nullptr && p->lm_rows != 1) ||
-      p->max_q_len < 1 || p->max_kv_len < p->max_q_len || H % 8 != 0)
-    return (int32_t)cudaErrorInvalidValue;
-  if (s->layers == nullptr || p->token_ids == nullptr || p->positions == nullptr || p->slot_mapping == nullptr ||
-      p->cu_seqlens_q == nullptr || p->cu_seqlens_k == nullptr || p->x == nullptr || p->x2 == nullptr || p->h == nullptr ||
-      p->q == nullptr || p->k == nullptr || p->v == nullptr || p->attn_out == nullptr || p->act == nullptr)
-    return (int32_t)cudaErrorInvalidValue;
-  if (T > GEMM_CHAIN_GROUPED_MAX_ROWS && p->gate_up == nullptr) return (int32_t)cudaErrorInvalidValue;
-  if (p->paged && (p->block_tables == nullptr || p->block_table_stride < 1 || p->num_blocks < 1)) return (int32_t)cudaErrorInvalidValue;
-  if (p->lm_rows == 1 && (p->last_rows == nullptr || p->h_last == nullptr || p->logits == nullptr || p->out_token == nullptr ||
-                          p->argmax_scratch == nullptr || (n <= 8 && p->q8_scratch == nullptr)))
-    return (int32_t)cudaErrorInvalidValue;
-  if (p->lm_rows == 2 && p->logits == nullptr) return (int32_t)cudaErrorInvalidValue;
-  if (p->dest_rows != nullptr && (p->runner_token_ids == nullptr || p->runner_context_lens == nullptr))
+  if (s->tp != nullptr || s->all_reduce != nullptr || s->layers == nullptr || p->k == nullptr || p->v == nullptr ||
+      (T > GEMM_CHAIN_GROUPED_MAX_ROWS && p->gate_up == nullptr) || (p->lm_rows == 1 && n <= 8 && p->q8_scratch == nullptr))
     return (int32_t)cudaErrorInvalidValue;
   if (const int32_t e = check_model(s)) return e;
   // the lm_head of n <= 8 last rows: the reference-shaped MMVQ launcher of its type

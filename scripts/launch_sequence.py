@@ -1,19 +1,21 @@
-"""Print the kernel launches of the Llama decode, verify and prompt steps and of the GPTQ decode and verify steps, one
-line per kernel node of a captured CUDA graph, in dependency order: kernel name, grid, block, dynamic shared memory,
-cluster dimensions (when set) and whether the incoming edge is programmatic (a PDL link).  Two builds of libmrs_b200.so
-that print the same lines enqueue the same launches, so a refactor of host-side launch code can be checked against its
-parent:
+"""Print the kernel launches of the Llama and GPTQ decode, verify and prompt steps (GPTQ also on act-order and AWQ
+checkpoints), one line per kernel node of a captured CUDA graph, in dependency order: kernel name, grid, block, dynamic
+shared memory, cluster dimensions (when set) and whether the incoming edge is programmatic (a PDL link).  Two builds of
+libmrs_b200.so that print the same lines enqueue the same launches, so a refactor of host-side launch code can be
+checked against its parent:
 
     python scripts/launch_sequence.py > new.txt
     python scripts/launch_sequence.py --lib /path/to/parent/libmrs_b200.so > old.txt
     diff old.txt new.txt
 
-The graph is read back through the driver API, as bench.py's count_graph_kernels does.  Synthetic seeded weights; the
-values computed do not matter here, only what is launched.  Needs a GPU."""
+The graph is read back through the driver API, as bench.py's count_graph_kernels does.  Synthetic seeded weights, and
+checkpoints written by the seeded writer of tests/test_gptq_checkpoint_host.py into a temporary directory; the values
+computed do not matter here, only what is launched.  Needs a GPU."""
 import argparse
 import ctypes
 import os
 import sys
+import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -160,16 +162,17 @@ def main():
 
     # ---- GPTQ decode steps: advance + W4A16 layer stack + dense lm_head + argmax, split plan (HND) and unsplit (vLLM)
     from mistralrs_b200 import gptq_model as G
-    gw = G.GptqWeights(G.GptqConfig.tiny_test(max_pos=4096), dev)
-    for layout in ("hnd", "vllm"):
-        for B in (4, 32):
-            run = G.GptqRunner(gw, batch=B, max_ctx=400, cache_layout=layout)
-            run.set_tokens([(5 * b + 3) % 500 for b in range(B)])
-            run.step()
-            report(f"gptq decode {layout} B={B}", capture(run.step))
-            del run
+
+    def gptq_decode(name, gw, layout, B, skip_mask=0):
+        run = G.GptqRunner(gw, batch=B, max_ctx=400, cache_layout=layout)
+        run.step_struct.skip_mask = skip_mask
+        run.set_tokens([(5 * b + 3) % 500 for b in range(B)])
+        run.step()
+        report(name, capture(run.step))
+        del run
+
     # ---- GPTQ verify steps (HND): advance_multi + W4A16 layer stack over B*q rows + lm_head + argmax + acceptance
-    for B, q in ((4, 4), (32, 8)):
+    def gptq_verify(name, gw, B, q):
         run = G.GptqRunner(gw, batch=B, max_ctx=400)
         run.set_tokens([(5 * b + 3) % 500 for b in range(B)])
         run.step()
@@ -177,9 +180,18 @@ def main():
         ver.sync_from_runner()
         ver.set_drafts([[(b + i) % 500 for i in range(q - 1)] for b in range(B)])
         ver.step()
-        report(f"gptq verify hnd B={B} q={q}", capture(ver.step))
+        report(name, capture(ver.step))
         del ver, run
-    del gw
+
+    gw = G.GptqWeights(G.GptqConfig.tiny_test(max_pos=4096), dev)
+    for layout in ("hnd", "vllm"):
+        for B in (4, 32):
+            gptq_decode(f"gptq decode {layout} B={B}", gw, layout, B)
+    # skip_mask bit 0: bench.py's linears-only graph; bit 2: plain stream order
+    gptq_decode("gptq decode hnd B=32 skip_mask=1", gw, "hnd", 32, skip_mask=1)
+    gptq_decode("gptq decode hnd B=32 skip_mask=4", gw, "hnd", 32, skip_mask=4)
+    for B, q in ((4, 4), (32, 8)):
+        gptq_verify(f"gptq verify hnd B={B} q={q}", gw, B, q)
 
     # ---- verify steps: advance_multi + layer stack + lm_head + argmax + acceptance
     for B, q in ((1, 4), (2, 4), (16, 4), (33, 8)):
@@ -193,37 +205,70 @@ def main():
         report(f"verify q4_k_m B={B} q={q}", capture(ver.step))
         del ver, run
 
-    # ---- prompt steps: only the mrs_llama_prefill_step call, the plan built eagerly before the capture
+    # ---- prompt steps: only the step call (pre.STEP), the plan built eagerly before the capture
     def prefill_case(name, pre, prompts, cached, tables, lm_rows, slots=None):
         p, _, plan = pre.make_plan(prompts, cached, tables, lm_rows, slots)    # plan: the device arrays p points into
 
         def call():
-            rc = pkg.lib().mrs_llama_prefill_step(ctypes.byref(pre.step_struct), ctypes.byref(p),
-                                                  ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+            rc = getattr(pkg.lib(), pre.STEP)(ctypes.byref(pre.step_struct), ctypes.byref(p),
+                                              ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
             if rc != 0:
-                raise RuntimeError(f"mrs_llama_prefill_step failed: cudaError {rc}")
+                raise RuntimeError(f"{pre.STEP} failed: cudaError {rc}")
         call()                                    # eager warm-up: module loads and kernel attributes
         report(name, capture(call))
         del plan
 
-    w = model("q4_k_m")
-    pre = M.LlamaPrefill(w, max_tokens=64)
-    prefill_case("prefill n=1 unpaged lm_rows=1", pre, [list(range(5, 25))], [0], [pre.table], 1)
-    runner = M.LlamaRunner(w, batch=12, max_ctx=128, pdl=True)
-    pre = M.LlamaPrefill(w, max_tokens=128, runner=runner)
-    prompts = [[(11 * i + j) % 500 for j in range(6 + i)] for i in range(9)]
-    tables = [list(runner.tables[i]) for i in range(9)]
-    pre.forward_batch([p[:4] for p in prompts[::3]], tables=tables[::3], final=False)
-    cached = [4 if i % 3 == 0 else 0 for i in range(9)]
-    prefill_case("prefill n=9 paged lm_rows=1 commit", pre, [p[c:] for p, c in zip(prompts, cached)], cached, tables, 1,
-                 slots=list(range(9)))
-    pre = M.LlamaPrefill(w, max_tokens=64)
-    own = [[1 + i] for i in range(4)]
-    prefill_case("prefill n=4 lm_rows=2", pre, [[(5 * i + j) % 500 for j in range(8)] for i in range(4)], [0] * 4, own, 2)
-    pre = M.LlamaPrefill(w, max_tokens=2400)
-    own = [list(range(1 + 18 * i, 19 + 18 * i)) for i in range(8)]
-    prefill_case("prefill n=8 T=2240 lm_rows=0", pre, [[(13 * i + j) % 500 for j in range(280)] for i in range(8)], [0] * 8,
-                 own, 0)
+    # the Llama prompt cases, repeated for the GPTQ prompt step: Prefill(weights, max_tokens=, runner=) and Runner(weights,
+    # batch=, max_ctx=) build the step's objects
+    def prefill_cases(tag, Prefill, Runner, w):
+        pre = Prefill(w, max_tokens=64)
+        prefill_case(f"{tag} n=1 unpaged lm_rows=1", pre, [list(range(5, 25))], [0], [pre.table], 1)
+        runner = Runner(w, batch=12, max_ctx=128)
+        pre = Prefill(w, max_tokens=128, runner=runner)
+        prompts = [[(11 * i + j) % 500 for j in range(6 + i)] for i in range(9)]
+        tables = [list(runner.tables[i]) for i in range(9)]
+        pre.forward_batch([p[:4] for p in prompts[::3]], tables=tables[::3], final=False)
+        cached = [4 if i % 3 == 0 else 0 for i in range(9)]
+        prefill_case(f"{tag} n=9 paged lm_rows=1 commit", pre, [p[c:] for p, c in zip(prompts, cached)], cached, tables, 1,
+                     slots=list(range(9)))
+        pre = Prefill(w, max_tokens=64)
+        own = [[1 + i] for i in range(4)]
+        prefill_case(f"{tag} n=4 lm_rows=2", pre, [[(5 * i + j) % 500 for j in range(8)] for i in range(4)], [0] * 4, own, 2)
+        pre = Prefill(w, max_tokens=2400)
+        own = [list(range(1 + 18 * i, 19 + 18 * i)) for i in range(8)]
+        prefill_case(f"{tag} n=8 T=2240 lm_rows=0", pre, [[(13 * i + j) % 500 for j in range(280)] for i in range(8)],
+                     [0] * 8, own, 0)
+
+    # the vLLM-layout GPTQ prompt step (unpaged only) with a commit into a vLLM-layout runner
+    def gptq_prefill_vllm(name, gw):
+        runner = G.GptqRunner(gw, batch=4, max_ctx=128, cache_layout="vllm")
+        pre = G.GptqPrefill(gw, max_tokens=64, runner=runner)
+        prefill_case(name, pre, [[(7 * i + j) % 500 for j in range(5 + 3 * i)] for i in range(4)], [0] * 4,
+                     [list(runner.tables[i]) for i in range(4)], 1, slots=list(range(4)))
+
+    prefill_cases("prefill", M.LlamaPrefill, lambda w, **kw: M.LlamaRunner(w, pdl=True, **kw), model("q4_k_m"))
+    prefill_cases("gptq prefill", G.GptqPrefill, G.GptqRunner, gw)
+    gptq_prefill_vllm("gptq prefill vllm n=4 unpaged lm_rows=1 commit", gw)
+    pre = G.GptqPrefill(gw, max_tokens=64, pdl=False)
+    prefill_case("gptq prefill n=1 unpaged lm_rows=1 pdl off", pre, [list(range(5, 25))], [0], [pre.table], 1)
+    del pre, gw
+
+    # ---- act-order GPTQ and AWQ checkpoints (the seeded writer of the host tests, into a temporary directory)
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_gptq_checkpoint_host import make_checkpoint
+    with tempfile.TemporaryDirectory() as tmp:
+        cfg = G.GptqConfig.tiny_test(max_pos=4096)
+        gw = G.GptqWeights.from_checkpoint(make_checkpoint(os.path.join(tmp, "act"), cfg, act_order=True), dev)
+        for layout in ("hnd", "vllm"):
+            gptq_decode(f"gptq act-order decode {layout} B=32", gw, layout, 32)
+        gptq_verify("gptq act-order verify hnd B=4 q=4", gw, 4, 4)
+        prefill_cases("gptq act-order prefill", G.GptqPrefill, G.GptqRunner, gw)
+        gptq_prefill_vllm("gptq act-order prefill vllm n=4 unpaged lm_rows=1 commit", gw)
+        del gw
+        gw = G.GptqWeights.from_checkpoint(make_checkpoint(os.path.join(tmp, "awq"), cfg, method="awq"), dev)
+        for layout in ("hnd", "vllm"):
+            gptq_decode(f"awq decode {layout} B=4", gw, layout, 4)
+        del gw
 
 
 if __name__ == "__main__":

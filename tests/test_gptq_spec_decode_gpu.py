@@ -417,15 +417,16 @@ def test_gptq_verifier_rejects_before_any_allocation(kw, k, msg):
 
 def test_gptq_verify_step_rejects_bad_arguments():
     """mrs_gptq_verify_step returns cudaErrorInvalidValue before any launch; every case differs from a well-formed
-    batch-16 step in one field (the pointers are never dereferenced)"""
+    two-layer batch-16 step in one field (the device pointers are never dereferenced)"""
     L = lib()
     bufs = (ctypes.c_int32 * 64)()
     p = lambda i: ctypes.addressof(bufs) + 4 * i
+    layers = (G._Layer * 2)()
 
     def call(q_len=4, ctx=True, acc=True, em=True, **fields):
         s = G._Step()
-        s.batch, s.head_dim, s.cache_layout, s.act_dtype, s.hidden = 16, 128, 1, 1, 4096
-        s.layers = ctypes.cast(p(48), ctypes.POINTER(G._Layer))
+        s.batch, s.n_layers, s.head_dim, s.cache_layout, s.act_dtype, s.hidden = 16, 2, 128, 1, 1, 4096
+        s.layers = ctypes.cast(layers, ctypes.POINTER(G._Layer))
         s.token_ids, s.out_token = p(0), p(8)
         for n, v in fields.items():
             setattr(s, n, v)
@@ -434,6 +435,6 @@ def test_gptq_verify_step_rejects_bad_arguments():
 
     bad = [dict(batch=0), dict(batch=257), dict(q_len=1), dict(q_len=9), dict(q_len=0), dict(cache_layout=0),
            dict(head_dim=96), dict(head_dim=256), dict(act_dtype=2), dict(act_dtype=3), dict(hidden=4092),
-           dict(layers=None), dict(out_token=p(0)), dict(ctx=False), dict(acc=False), dict(em=False)]
+           dict(layers=None), dict(n_layers=0), dict(out_token=p(0)), dict(ctx=False), dict(acc=False), dict(em=False)]
     for kw in bad:
         assert call(**kw) == 1, kw
